@@ -8,8 +8,7 @@ import ctypes
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# DISCO_B200_LIB selects another build of the same library (scripts/build_variants.py: A/B of kernel tunings)
-LIB_PATH = os.environ.get("DISCO_B200_LIB") or os.path.join(_HERE, "libdisco_b200.so")
+LIB_PATH = os.path.join(_HERE, "libdisco_b200.so")
 
 c_int, c_void_p, c_size_t, c_float, c_double = (ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t,
                                                 ctypes.c_float, ctypes.c_double)

@@ -85,11 +85,6 @@ DISCO_DEV void tma_load_1d(void* dst_smem, const void* src_gmem, uint32_t bytes,
         "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar))
         : "memory");
 }
-// Bulk prefetch of a contiguous global range into L2 (no shared-memory destination, no completion tracking):
-// hides the DRAM latency of a later tma_load_1d of the same range.  src 16-byte aligned, bytes a multiple of 16.
-DISCO_DEV void tma_prefetch_l2(const void* src_gmem, uint32_t bytes) {
-    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src_gmem), "r"(bytes) : "memory");
-}
 DISCO_DEV void named_bar_sync(int id, int nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }

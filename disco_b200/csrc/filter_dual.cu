@@ -9,35 +9,14 @@
 #include "common.cuh"
 #include "kernels.h"
 
-// tuning knobs (scripts/build_variants.py builds alternatives for A/B runs; on an H100 none of the fd_ variants beats
-// these defaults by more than the run-to-run spread, and a third resident block (MINB 3) is 35 % slower)
-#ifndef DISCO_FD_UF
-#define DISCO_FD_UF 4          // frames per thread and register buffer (frame-major output)
-#endif
-#ifndef DISCO_FD_MINB
-#define DISCO_FD_MINB 2        // resident CTAs per SM the register allocation aims for
-#endif
-#ifndef DISCO_FD_WANT
-#define DISCO_FD_WANT 32       // CTAs per SM the time split aims for (equal-sized CTAs: more waves, shorter tail)
-#endif
-#ifndef DISCO_FD_STCS
-#define DISCO_FD_STCS 1        // 1: streaming (evict-first) stores for the three outputs
-#endif
-
 namespace disco {
 
-DISCO_DEV void fd_store(float2* p, float2 v) {
-#if DISCO_FD_STCS
-    __stcs(p, v);
-#else
-    *p = v;
-#endif
-}
-
+// Two resident CTAs per SM (a third is 35 % slower on an H100), 4 frames per thread and register buffer, streaming
+// stores for the three outputs: no other setting beat these by more than the run-to-run spread (DESIGN.md 4.1).
 template <int C, bool OUT_FT>
-__global__ void __launch_bounds__(256, DISCO_FD_MINB) filter_dual_kernel(DualFilterArgs a, int frames_per_slab) {
+__global__ void __launch_bounds__(256, 2) filter_dual_kernel(DualFilterArgs a, int frames_per_slab) {
     constexpr int TS = 8;                         // warps per block = time ways
-    constexpr int UF = OUT_FT ? 4 : DISCO_FD_UF;  // frames per thread and buffer
+    constexpr int UF = 4;                         // frames per thread and buffer
     __shared__ float2 tile[OUT_FT ? 3 : 1][OUT_FT ? 32 : 1][33];
     const int lane = threadIdx.x & 31, wrp = threadIdx.x >> 5;
     const int grp = blockIdx.y;
@@ -87,9 +66,9 @@ __global__ void __launch_bounds__(256, DISCO_FD_MINB) filter_dual_kernel(DualFil
             const float2 zn = csub(r, z);
             if (!OUT_FT) {
                 if (tt < t_end) {
-                    fd_store(a.z + go + (size_t)tt * F + f, z);
-                    if (a.zn) fd_store(a.zn + go + (size_t)tt * F + f, zn);
-                    fd_store(a.yf + go + (size_t)tt * F + f, yf);
+                    st_stream(a.z + go + (size_t)tt * F + f, z);
+                    if (a.zn) st_stream(a.zn + go + (size_t)tt * F + f, zn);
+                    st_stream(a.yf + go + (size_t)tt * F + f, yf);
                 }
             } else {
                 const int tl = wrp * UF + u;
@@ -130,12 +109,10 @@ __global__ void __launch_bounds__(256, DISCO_FD_MINB) filter_dual_kernel(DualFil
 template <int C>
 static cudaError_t launch_c(const DualFilterArgs& a, int sm, cudaStream_t st) {
     const int fblocks = (a.F + 31) / 32;
-    // enough CTAs to fill the machine: split time into slabs (multiples of 32 frames) when groups are few
-    int slabs = 1;
-    const int want = sm * DISCO_FD_WANT;
-    while (fblocks * a.n_grp * slabs < want && (a.T + slabs - 1) / slabs > 64) slabs *= 2;
-    const int fps = ((a.T + slabs - 1) / slabs + 31) / 32 * 32;
-    slabs = (a.T + fps - 1) / fps;
+    // enough CTAs to fill the machine: split time into slabs when groups are few.  32 CTAs per SM: the CTAs are
+    // equal-sized, so more waves make a shorter tail
+    const int fps = filter_slab_frames(a.T, fblocks * a.n_grp, sm * 32);
+    const int slabs = (a.T + fps - 1) / fps;
     if (a.n_grp > 65535 || slabs > 65535) return cudaErrorInvalidConfiguration;
     dim3 grid(fblocks, a.n_grp, slabs);
     if (a.out_ft)

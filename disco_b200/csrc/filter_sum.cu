@@ -12,14 +12,6 @@
 
 namespace disco {
 
-DISCO_DEV const float2* cat_channel_fs(const CatArgs& in, int grp, int d) {
-    if (d < in.C) return in.Y + ((size_t)grp * in.C + d) * in.T * in.F;
-    const int b = grp / in.n_sel, k = in.sel[grp % in.n_sel];
-    int j = d - in.C;
-    if (j >= k) ++j;
-    return in.Z + ((size_t)b * in.z_sb + (size_t)j * in.z_sk) * in.T * in.F;
-}
-
 template <int D>
 __global__ void __launch_bounds__(256) filter_sum_kernel(FilterArgs a, int frames_per_slab) {
     __shared__ float2 tile_o[32][33];
@@ -40,9 +32,9 @@ __global__ void __launch_bounds__(256) filter_sum_kernel(FilterArgs a, int frame
     for (int d = 0; d < D; ++d) {
         float2 v = a.W[((size_t)grp * F + fc) * D + d];
         w[d] = a.conj_w ? cconj(v) : v;
-        ch[d] = cat_channel_fs(a.in, grp, d) + fc;
+        ch[d] = cat_channel(a.in, grp, d) + fc;
     }
-    const float2* refch = cat_channel_fs(a.in, grp, a.ref) + fc;
+    const float2* refch = cat_channel(a.in, grp, a.ref) + fc;
 
     // Software pipeline (small D): the 4 frames this warp owns in the NEXT 32-frame tile are loaded
     // before the current ones are consumed, keeping 4 D loads per thread in flight.
@@ -131,9 +123,9 @@ __global__ void __launch_bounds__(256, (D <= 4 ? 2 : 1)) filter_sum_tf_kernel(Fi
     for (int d = 0; d < D; ++d) {
         const float2 v = a.W[((size_t)grp * F + f) * D + d];
         w[d] = a.conj_w ? cconj(v) : v;
-        ch[d] = cat_channel_fs(a.in, grp, d) + f;
+        ch[d] = cat_channel(a.in, grp, d) + f;
     }
-    const float2* refch = cat_channel_fs(a.in, grp, a.ref) + f;
+    const float2* refch = cat_channel(a.in, grp, a.ref) + f;
     float2* out = a.out + (size_t)grp * T * F + f;
     float2* res = a.resid ? a.resid + (size_t)grp * T * F + f : nullptr;
     constexpr int TS = 8;                         // warps per block = time ways
@@ -174,12 +166,9 @@ __global__ void __launch_bounds__(256, (D <= 4 ? 2 : 1)) filter_sum_tf_kernel(Fi
 template <int D>
 static cudaError_t launch_d(const FilterArgs& a, cudaStream_t st) {
     const int fblocks = (a.in.F + 31) / 32;
-    // enough CTAs to fill the machine: split time into slabs (multiples of 32 frames) when groups are few
-    int slabs = 1;
-    const int want = sm_count() * 4;
-    while (fblocks * a.in.n_grp * slabs < want && (a.in.T + slabs - 1) / slabs > 64) slabs *= 2;
-    int fps = ((a.in.T + slabs - 1) / slabs + 31) / 32 * 32;
-    slabs = (a.in.T + fps - 1) / fps;
+    // enough CTAs to fill the machine (4 per SM): split time into slabs when groups are few
+    const int fps = filter_slab_frames(a.in.T, fblocks * a.in.n_grp, sm_count() * 4);
+    const int slabs = (a.in.T + fps - 1) / fps;
     dim3 grid(fblocks, a.in.n_grp, slabs);
     if (!a.out_ft) {
         if (D <= 4 && a.in.F == 257)

@@ -32,8 +32,34 @@ cudaError_t launch_scm_finalize(const float* part, float2* Rss, float2* Rnn, int
                                 int tiles_per_grp, int n_cta, int C, int F, int T, int n_set, int set, cudaStream_t st);
 int stft_tile_frames(int n_fft, int C);
 int stft_tiles_per_grp(int n_fft, int C, int T);
-int stft_slots_per_grp(int n_grp, int tiles_per_grp, int n_cta);
-int stft_cta_of_tile_host(long long i, long long total, int nb);
+
+// Segment layout of the partial sums (StftArgs::part).  The total = n_grp * tiles_per_grp tiles are cut into
+// n_cta contiguous ranges, CTA b owning [total * b / n_cta, total * (b + 1) / n_cta); the CTAs whose range meets
+// group g write its slots 0, 1, ... in CTA order, and the finalize kernel and the solver sum them in that order.
+// first CTA whose tile range contains tile i
+__host__ __device__ __forceinline__ int cta_of_tile(long long i, long long total, int n_cta) {
+    int b = (int)((i * n_cta) / total);
+    if (b >= n_cta) b = n_cta - 1;
+    while (b + 1 < n_cta && total * (b + 1) / n_cta <= i) ++b;
+    while (b > 0 && total * b / n_cta > i) --b;
+    return b;
+}
+// the CTAs that wrote the slots of group g: first .. last, in slot order
+struct SegSlots {
+    int first, last;
+    __host__ __device__ __forceinline__ int count() const { return last - first + 1; }
+};
+__host__ __device__ __forceinline__ SegSlots seg_slots(int g, int tiles_per_grp, long long total, int n_cta) {
+    return {cta_of_tile((long long)g * tiles_per_grp, total, n_cta),
+            cta_of_tile((long long)(g + 1) * tiles_per_grp - 1, total, n_cta)};
+}
+// Upper bound on the number of CTAs whose tile range intersects one group (slots_per_grp).
+inline int stft_slots_per_grp(int n_grp, int tiles_per_grp, int n_cta) {
+    const long long total = (long long)n_grp * tiles_per_grp;
+    const long long min_range = total / n_cta;   // every CTA owns floor or ceil(total / n_cta) tiles
+    if (min_range == 0) return tiles_per_grp + 1;
+    return (int)(tiles_per_grp / min_range) + 2;
+}
 
 // Step-2 style input: group g = (utterance b, node k) sees D = C + K - 1 channels:
 // its own C microphone spectra, then the compressed signals z of the other nodes in node
@@ -50,6 +76,16 @@ struct CatArgs {
     int n_sel;         // nodes covered by this launch (K when all nodes have C microphones)
     int sel[16];       // their node indices, ascending
 };
+
+// Plane [T][F] of channel d of group grp: d < C is an own microphone, d >= C the compressed signal of node j, the
+// other nodes in order, skipping the group's own node (tango.py:153-155).
+__device__ __forceinline__ const float2* cat_channel(const CatArgs& in, int grp, int d) {
+    if (d < in.C) return in.Y + ((size_t)grp * in.C + d) * in.T * in.F;
+    const int b = grp / in.n_sel, k = in.sel[grp % in.n_sel];
+    int j = d - in.C;
+    if (j >= k) ++j;
+    return in.Z + ((size_t)b * in.z_sb + (size_t)j * in.z_sk) * in.T * in.F;
+}
 
 struct ScmArgs {
     CatArgs in;
@@ -75,7 +111,7 @@ struct SolveArgs {
     int type;            // 0 gevd, 1 r1-mwf, 2 mwf
     int rank;            // gevd: number of generalised eigenpairs kept; <= 0 or >= D means full
     double mu;
-    // optional: read the matrices straight from the fused STFT+SCM kernel's segment partial sums
+    // optional, D <= 4 only: read the matrices straight from the fused STFT+SCM kernel's segment partial sums
     // (skips scm_finalize); matrix idx = (set * n_grp + grp) * F + f, n_mat = n_set * n_grp * F
     const float* part;   // [n_grp][slots_per_grp][n_set][2 D^2][F] or null
     int slots_per_grp, tiles_per_grp, n_cta, F;
@@ -95,6 +131,14 @@ struct FilterArgs {
 };
 cudaError_t launch_filter_sum(const FilterArgs& a, cudaStream_t st);
 cudaError_t launch_filter_sum_multi(const FilterArgs& a, cudaStream_t st);   // K > 1, all nodes, TF output
+
+// Time split of the filter launches (grid.z): frames per slab, a multiple of 32.  When the ctas = bin blocks x
+// groups are fewer than want_ctas, the T frames are halved into more slabs while a slab keeps more than 64 frames.
+inline int filter_slab_frames(int T, int ctas, int want_ctas) {
+    int slabs = 1;
+    while (ctas * slabs < want_ctas && (T + slabs - 1) / slabs > 64) slabs *= 2;
+    return ((T + slabs - 1) / slabs + 31) / 32 * 32;
+}
 
 // Single-node groups, both filters in one pass over Y (filter_dual.cu): z = w1^H y, zn = y[ref] - z, yf = w2^H y
 struct DualFilterArgs {

@@ -16,14 +16,6 @@
 
 namespace disco {
 
-DISCO_DEV const float2* online_channel(const CatArgs& in, int grp, int d) {
-    if (d < in.C) return in.Y + ((size_t)grp * in.C + d) * in.T * in.F;
-    const int b = grp / in.n_sel, k = in.sel[grp % in.n_sel];
-    int j = d - in.C;
-    if (j >= k) ++j;  // skip own compressed signal (tango.py:153-155)
-    return in.Z + ((size_t)b * in.z_sb + (size_t)j * in.z_sk) * in.T * in.F;
-}
-
 constexpr int kOnlineBY = 4;   // blocks of frames per CTA (threadIdx.y)
 
 template <int D>
@@ -37,7 +29,7 @@ __global__ void __launch_bounds__(32 * kOnlineBY) scm_blocks_kernel(OnlineArgs a
     const int t0 = j * a.P, t1 = min(T, t0 + a.P);          // frames [t0, t1)
     const float2* ch[D];
 #pragma unroll
-    for (int d = 0; d < D; ++d) ch[d] = online_channel(a.in, grp, d) + f;
+    for (int d = 0; d < D; ++d) ch[d] = cat_channel(a.in, grp, d) + f;
     const float* mrow = a.mask ? a.mask + (size_t)grp * T * F + f : nullptr;
 
     float2 ps[G::NPP], pn[G::NPP];
@@ -103,7 +95,7 @@ __global__ void __launch_bounds__(32 * kOnlineBY) filter_sum_blocks_kernel(Onlin
     }
     const float2* ch[D];
 #pragma unroll
-    for (int d = 0; d < D; ++d) ch[d] = online_channel(a.in, grp, d) + f;
+    for (int d = 0; d < D; ++d) ch[d] = cat_channel(a.in, grp, d) + f;
     for (int t = t0; t < t1; ++t) {
         float2 z = make_float2(0.f, 0.f), yr = make_float2(0.f, 0.f);
 #pragma unroll

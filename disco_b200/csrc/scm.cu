@@ -14,74 +14,39 @@
 // At D <= 4 the 2 x D(D+1)/2 accumulators AND two software-pipelined frames of operands fit in
 // registers; the TW time-ways are reduced through shared memory at the end (fixed order ->
 // deterministic), then scaled by 1/T and written with their conjugate mirrors.
-#include "common.cuh"
 #include "kernels.h"
+#include "scm_core.cuh"
 
 namespace disco {
 
 template <int D>
 struct ScmGeom {
-    static constexpr int NPAIR = D * (D + 1) / 2;
-    static constexpr int NPART = 1;   // all pairs in one thread (the partitioned variants live in scm_wide.cu)
-    static constexpr int NPP = (NPAIR + NPART - 1) / NPART;  // pairs per partition
-    static constexpr int TW = 8 / NPART;
-    static constexpr int THREADS = 256;
+    static constexpr int NPAIR = D * (D + 1) / 2;   // all pairs in one thread
+    static constexpr int TW = 8;                    // time-ways (warps)
+    static constexpr int THREADS = 32 * TW;
 };
 
-// pair index -> (i, j), i <= j, row-major over the upper triangle (compile-time)
-template <int D>
-__host__ __device__ constexpr int pair_i(int p) {
-    int i = 0, n = D;
-    while (p >= n) {
-        p -= n;
-        --n;
-        ++i;
-    }
-    return i;
-}
-template <int D>
-__host__ __device__ constexpr int pair_j(int p) {
-    int i = 0, n = D;
-    while (p >= n) {
-        p -= n;
-        --n;
-        ++i;
-    }
-    return i + p;
-}
-
-DISCO_DEV const float2* cat_channel(const CatArgs& in, int grp, int d) {
-    if (d < in.C) return in.Y + ((size_t)grp * in.C + d) * in.T * in.F;
-    const int b = grp / in.n_sel, k = in.sel[grp % in.n_sel];
-    int j = d - in.C;
-    if (j >= k) ++j;  // skip own compressed signal (tango.py:153-155)
-    return in.Z + ((size_t)b * in.z_sb + (size_t)j * in.z_sk) * in.T * in.F;
-}
-
-// compile-time recursion over the pairs of one partition: (i, j) are constants, so y[] and the
-// accumulators stay in registers
-template <int D, int PART, int Q>
+// compile-time recursion over the pairs: (i, j) are constants, so y[] and the accumulators stay in registers
+template <int D, int Q>
 struct PairAcc {
     using G = ScmGeom<D>;
-    static DISCO_DEV void run(const float2 (&y)[D], float wa, float wb, float2 (&ps)[G::NPP], float2 (&pn)[G::NPP]) {
-        if constexpr (Q < G::NPP) {
-            constexpr int pidx = Q * G::NPART + PART;
-            if constexpr (pidx < G::NPAIR) {
-                constexpr int i = pair_i<D>(pidx), j = pair_j<D>(pidx);
-                const float2 op = cmulc(y[i], y[j]);
-                ps[Q] = cfma_r(wa, op, ps[Q]);
-                pn[Q] = cfma_r(wb, op, pn[Q]);
-            }
-            PairAcc<D, PART, Q + 1>::run(y, wa, wb, ps, pn);
+    static DISCO_DEV void run(const float2 (&y)[D], float wa, float wb, float2 (&ps)[G::NPAIR],
+                              float2 (&pn)[G::NPAIR]) {
+        if constexpr (Q < G::NPAIR) {
+            constexpr int i = tri_i<D>(Q), j = tri_j<D>(Q);
+            const float2 op = cmulc(y[i], y[j]);
+            ps[Q] = cfma_r(wa, op, ps[Q]);
+            pn[Q] = cfma_r(wb, op, pn[Q]);
+            PairAcc<D, Q + 1>::run(y, wa, wb, ps, pn);
         }
     }
 };
 
 // FC > 0: the number of bins is the compile-time constant FC (257 for the 512-point STFT), which turns
 // the row-stride multiplications of every address into immediates; FC == 0: runtime F.
-template <int D, int PART, bool ZF, int FC>
+template <int D, bool ZF, int FC>
 DISCO_DEV void scm_accumulate(const ScmArgs& a, int grp, int f, bool active, int tw,
-                              float2 (&ps)[ScmGeom<D>::NPP], float2 (&pn)[ScmGeom<D>::NPP]) {
+                              float2 (&ps)[ScmGeom<D>::NPAIR], float2 (&pn)[ScmGeom<D>::NPAIR]) {
     using G = ScmGeom<D>;
     const int T = a.in.T;
     const int F = FC ? FC : a.in.F;
@@ -91,20 +56,19 @@ DISCO_DEV void scm_accumulate(const ScmArgs& a, int grp, int f, bool active, int
     const float* mrow = a.mask ? (a.mask_ft ? a.mask + ((size_t)grp * F + f) * T : a.mask + (size_t)grp * T * F + f)
                                : nullptr;
     const int mstride = a.mask_ft ? 1 : F;
-    // fused step-1 filter (only the first pair-partition writes; K == 1 so D == C)
-    constexpr bool zfuse = ZF && (PART == 0);
+    // fused step-1 filter (K == 1 so D == C)
     float2 w1[D];
-    if (zfuse) {
+    if (ZF) {
 #pragma unroll
         for (int d = 0; d < D; ++d) w1[d] = cconj(a.W1[((size_t)grp * F + f) * D + d]);
     }
-    float2* zrow = zfuse ? a.z_out + (size_t)grp * T * F + f : nullptr;
-    float2* znrow = (zfuse && a.zn_out) ? a.zn_out + (size_t)grp * T * F + f : nullptr;
+    float2* zrow = ZF ? a.z_out + (size_t)grp * T * F + f : nullptr;
+    float2* znrow = (ZF && a.zn_out) ? a.zn_out + (size_t)grp * T * F + f : nullptr;
     const int ref = a.ref;
     auto point = [&](const float2 (&y)[D], float m, int t) {
         const float wa = m * m, wb = mrow ? (1.f - m) * (1.f - m) : 0.f;
-        PairAcc<D, PART, 0>::run(y, wa, wb, ps, pn);
-        if (zfuse && active) {
+        PairAcc<D, 0>::run(y, wa, wb, ps, pn);
+        if (ZF && active) {
             float2 z = cfma(w1[0], y[0], make_float2(0.f, 0.f));
 #pragma unroll
             for (int d = 1; d < D; ++d) z = cfma(w1[d], y[d], z);
@@ -177,37 +141,35 @@ DISCO_DEV void scm_accumulate(const ScmArgs& a, int grp, int f, bool active, int
 template <int D, bool ZF, int FC>
 __global__ void __launch_bounds__(ScmGeom<D>::THREADS, 2) masked_scm_kernel(ScmArgs a) {
     using G = ScmGeom<D>;
-    extern __shared__ float2 red[];  // [NPART][NPP][2][32]
+    extern __shared__ float2 red[];  // [NPAIR][2][32]
     const int lane = threadIdx.x & 31;
-    const int part = (threadIdx.x >> 5) % G::NPART;
-    const int tw = threadIdx.x / (32 * G::NPART);
+    const int tw = threadIdx.x >> 5;
     const int grp = blockIdx.y;
     const int f = blockIdx.x * 32 + lane;
     const bool active = f < a.in.F;
     const int fc = active ? f : a.in.F - 1;
 
-    float2 ps[G::NPP], pn[G::NPP];
+    float2 ps[G::NPAIR], pn[G::NPAIR];
 #pragma unroll
-    for (int q = 0; q < G::NPP; ++q) ps[q] = pn[q] = make_float2(0.f, 0.f);
+    for (int q = 0; q < G::NPAIR; ++q) ps[q] = pn[q] = make_float2(0.f, 0.f);
 
-    scm_accumulate<D, 0, ZF, FC>(a, grp, fc, active, tw, ps, pn);
+    scm_accumulate<D, ZF, FC>(a, grp, fc, active, tw, ps, pn);
 
     // reduce the TW time-ways in fixed order: way w adds into way 0 through shared memory
-    float2* mine = red + (size_t)part * G::NPP * 2 * 32;
     for (int w = 1; w < G::TW; ++w) {
         if (tw == w) {
 #pragma unroll
-            for (int q = 0; q < G::NPP; ++q) {
-                mine[(q * 2 + 0) * 32 + lane] = ps[q];
-                mine[(q * 2 + 1) * 32 + lane] = pn[q];
+            for (int q = 0; q < G::NPAIR; ++q) {
+                red[(q * 2 + 0) * 32 + lane] = ps[q];
+                red[(q * 2 + 1) * 32 + lane] = pn[q];
             }
         }
         __syncthreads();
         if (tw == 0) {
 #pragma unroll
-            for (int q = 0; q < G::NPP; ++q) {
-                ps[q] = cadd(ps[q], mine[(q * 2 + 0) * 32 + lane]);
-                pn[q] = cadd(pn[q], mine[(q * 2 + 1) * 32 + lane]);
+            for (int q = 0; q < G::NPAIR; ++q) {
+                ps[q] = cadd(ps[q], red[(q * 2 + 0) * 32 + lane]);
+                pn[q] = cadd(pn[q], red[(q * 2 + 1) * 32 + lane]);
             }
         }
         __syncthreads();
@@ -216,26 +178,24 @@ __global__ void __launch_bounds__(ScmGeom<D>::THREADS, 2) masked_scm_kernel(ScmA
         const float inv_T = 1.0f / (float)a.in.T;
         float2* Rs = a.Rss + ((size_t)grp * a.in.F + f) * D * D;
         float2* Rn = a.Rnn + ((size_t)grp * a.in.F + f) * D * D;
+        // scaled pairs with their conjugate mirrors, as store_pairs (scm_core.cuh) writes them; calling store_pairs or
+        // taking (i, j) from tri_i / tri_j here makes nvcc reschedule the whole kernel, so the epilogue stays as it is
 #pragma unroll
-        for (int q = 0; q < G::NPP; ++q) {
-            // `part` is runtime here; recover (i, j) arithmetically (tiny epilogue, not the hot loop)
-            int pidx = q * G::NPART + part;
-            if (pidx < G::NPAIR) {
-                int i = 0, n = D, pp = pidx;
-                while (pp >= n) {
-                    pp -= n;
-                    --n;
-                    ++i;
-                }
-                const int j = i + pp;
-                float2 s = cscale(ps[q], inv_T), nn = cscale(pn[q], inv_T);
-                if (i == j) s.y = 0.f, nn.y = 0.f;
-                Rs[i * D + j] = s;
-                Rn[i * D + j] = nn;
-                if (i != j) {
-                    Rs[j * D + i] = cconj(s);
-                    Rn[j * D + i] = cconj(nn);
-                }
+        for (int q = 0; q < G::NPAIR; ++q) {
+            int i = 0, n = D, pp = q;
+            while (pp >= n) {
+                pp -= n;
+                --n;
+                ++i;
+            }
+            const int j = i + pp;
+            float2 s = cscale(ps[q], inv_T), nn = cscale(pn[q], inv_T);
+            if (i == j) s.y = 0.f, nn.y = 0.f;
+            Rs[i * D + j] = s;
+            Rn[i * D + j] = nn;
+            if (i != j) {
+                Rs[j * D + i] = cconj(s);
+                Rn[j * D + i] = cconj(nn);
             }
         }
     }
@@ -244,7 +204,7 @@ __global__ void __launch_bounds__(ScmGeom<D>::THREADS, 2) masked_scm_kernel(ScmA
 template <int D, bool ZF, int FC>
 static cudaError_t launch_dzf(const ScmArgs& a, cudaStream_t st) {
     using G = ScmGeom<D>;
-    const size_t smem = (size_t)G::NPART * G::NPP * 2 * 32 * sizeof(float2);
+    const size_t smem = (size_t)G::NPAIR * 2 * 32 * sizeof(float2);
     auto kern = masked_scm_kernel<D, ZF, FC>;
     if (smem > 48 * 1024) {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);

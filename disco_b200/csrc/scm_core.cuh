@@ -1,6 +1,7 @@
 // Shared pieces of the wide-channel SCM kernels (scm_wide.cu, mid_multi.cu): everything a CTA that owns
 // (group, 32-bin block) needs to stream tiles of spectra through shared memory and accumulate the
-// Hermitian pairs of  sum_t m^2 x x^H  and  sum_t (1-m)^2 x x^H  in registers.
+// Hermitian pairs of  sum_t m^2 x x^H  and  sum_t (1-m)^2 x x^H  in registers.  The pair index
+// (tri_i / tri_j) also serves scm.cu, and the matrix store (store_pairs) online.cu.
 //
 //  * cp.async (LDGSTS) 8-byte copies fill a ring of shared-memory stages; out-of-range frames and bins
 //    are zero-filled by the copy itself (src-size 0), so the accumulation loops carry no predicates

@@ -31,14 +31,6 @@ struct WideCfg {
     static_assert(SL % NPART == 0 || NPART > 2, "fused z output: the slots of a way are dealt to its partitions");
 };
 
-DISCO_DEV const float2* wide_channel(const CatArgs& in, int grp, int d) {
-    if (d < in.C) return in.Y + ((size_t)grp * in.C + d) * in.T * in.F;
-    const int b = grp / in.n_sel, k = in.sel[grp % in.n_sel];
-    int j = d - in.C;
-    if (j >= k) ++j;  // skip own compressed signal (tango.py:153-155)
-    return in.Z + ((size_t)b * in.z_sb + (size_t)j * in.z_sk) * in.T * in.F;
-}
-
 // one way's slots of one tile: operands from shared memory, optional fused z = w1^H y output
 template <int D, int NPART, int TW, int TS, int NS, bool ZF, int PART>
 DISCO_DEV void wide_tile(const ScmArgs& a, const float2* yb, const float* mb, const float2* w1s, bool has_mask,
@@ -89,7 +81,7 @@ __global__ void __launch_bounds__(32 * NPART * TW, MINB) masked_scm_wide_kernel(
     const int ntile = (T + tspan - 1) / tspan;
     const bool has_mask = a.mask != nullptr;
 
-    if (threadIdx.x < D) plane[threadIdx.x] = wide_channel(a.in, grp, threadIdx.x);
+    if (threadIdx.x < D) plane[threadIdx.x] = cat_channel(a.in, grp, threadIdx.x);
     if (ZF)
         for (int d = warp; d < D; d += NW) w1s[d * 32 + lane] = cconj(a.W1[((size_t)grp * F + lg.fcol) * D + d]);
     __syncthreads();

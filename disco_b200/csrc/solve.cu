@@ -26,11 +26,6 @@
 #include "common.cuh"
 #include "kernels.h"
 
-// 1: deal the entries of the Hermitian squaring to all G lanes of a group (see g_top_eigpair); experimental, off
-#ifndef DISCO_SOLVE_SPREAD
-#define DISCO_SOLVE_SPREAD 0
-#endif
-
 namespace disco {
 
 struct cd {
@@ -229,65 +224,10 @@ DISCO_DEV double g_top_eigpair(const cd* A, cd* B, int l, unsigned gm, cd* v_out
         for (int j = 0; j < D; ++j) B[l * P + j] = it * A[l * P + j];
     }
     __syncwarp(gm);
-    // B is Hermitian, so is B^2: only the NE = D (D + 1) / 2 entries (i <= j) are computed, each stored with its
-    // conjugate mirror.  Two ways of dealing them to the group's G lanes:
-    //  * SPREAD (-DDISCO_SOLVE_SPREAD=1; D = 5, 6, 9, 10, ...: G is well above D): entry e goes to lane e mod G, so
-    //    the lanes beyond D work too -- 3 entries per lane instead of 5 at D = 9.  Written at the end of round 2
-    //    and NOT yet run on a GPU, hence compiled out by default (the default build's SASS is unchanged);
-    //  * otherwise lane l owns the H = D/2 + 1 entries (l, (l + s) mod D) of its row (every unordered pair has an
-    //    owner; for even D the pairs at distance D/2 have two owners that compute and store the same numbers).
+    // B is Hermitian, so is B^2: only the entries i <= j are computed, each stored with its conjugate mirror.  Lane l
+    // owns the H = D/2 + 1 entries (l, (l + s) mod D) of its row (every unordered pair has an owner; for even D the
+    // pairs at distance D/2 have two owners that compute and store the same numbers).
     constexpr int H = D / 2 + 1;
-    constexpr int NE = D * (D + 1) / 2, EPL = (NE + G - 1) / G;
-    constexpr bool SPREAD = DISCO_SOLVE_SPREAD && EPL < H;
-    if constexpr (SPREAD) {
-        int ei[EPL], ej[EPL];
-#pragma unroll
-        for (int s = 0; s < EPL; ++s) {
-            int e = l + s * G, i = 0;
-            if (e >= NE) {
-                ei[s] = -1;
-                ej[s] = 0;
-                continue;
-            }
-            while (e >= D - i) {
-                e -= D - i;
-                ++i;
-            }
-            ei[s] = i;
-            ej[s] = i + e;
-        }
-        for (int iter = 0; iter < 40; ++iter) {
-            cd c[EPL];
-            double fro = 0.0, dg = 0.0;
-#pragma unroll
-            for (int s = 0; s < EPL; ++s) {
-                c[s] = mk(0.0, 0.0);
-                if (ei[s] < 0) continue;
-                const cd *ri = B + ei[s] * P, *rj = B + ej[s] * P;      // B[k][j] = conj(B[j][k]): two row reads
-                for (int k = 0; k < D; ++k) c[s] = c[s] + ri[k] * conj(rj[k]);
-                if (ei[s] == ej[s]) {
-                    c[s].y = 0.0;
-                    dg += c[s].x;
-                    fro += c[s].x * c[s].x;
-                } else {
-                    fro += 2.0 * norm2(c[s]);
-                }
-            }
-            const double trc = gsum<G>(dg, gm);      // tr(B^2) = ||B||_F^2 of the previous iterate (<= 1)
-            const double fr2 = gsum<G>(fro, gm);     // ||B^2||_F^2
-            __syncwarp(gm);                          // everyone has finished reading B
-            const double it = 1.0 / trc;
-#pragma unroll
-            for (int s = 0; s < EPL; ++s) {
-                if (ei[s] < 0) continue;
-                const cd v = it * c[s];
-                B[ei[s] * P + ej[s]] = v;
-                if (ei[s] != ej[s]) B[ej[s] * P + ei[s]] = conj(v);
-            }
-            __syncwarp(gm);
-            if (1.0 - fr2 / (trc * trc) <= 1e-14) break;   // new iterate is rank one (group-uniform)
-        }
-    } else {
     int col[H];
 #pragma unroll
     for (int s = 0; s < H; ++s) col[s] = (l + s) % D;
@@ -327,7 +267,6 @@ DISCO_DEV double g_top_eigpair(const cd* A, cd* B, int l, unsigned gm, cd* v_out
         __syncwarp(gm);
         if (1.0 - fr2 / (trc * trc) <= 1e-14) break;   // new iterate is rank one (group-uniform)
     }
-    }
     // B ~ v v^H: take the column with the largest diagonal, normalise
     int jm = 0;
     double dmax = B[0].x;
@@ -361,41 +300,7 @@ DISCO_DEV void g_load_herm(const float2* __restrict__ R, cd* M, int l) {
         }
 }
 
-// Lane l builds row l from the fused STFT+SCM kernel's partial sums: accumulator layout
-// [D diagonals][D(D-1)/2 x (re, im) upper pairs, row-major], slots summed in order, scaled by 1/T
-// in float32 (the same arithmetic as scm_finalize_kernel: both routes give identical matrices).
 template <int D>
-DISCO_DEV void g_load_part(const float* __restrict__ q, int n_slot, size_t slot_stride, int F, float inv_T, cd* M,
-                           int l) {
-    constexpr int P = SolveGeom<D>::P;
-    if (l >= D) return;
-    for (int j = 0; j < D; ++j) {
-        const int i0 = l < j ? l : j, j0 = l < j ? j : l;
-        float re = 0.f, im = 0.f;
-        if (i0 == j0) {
-            for (int sl = 0; sl < n_slot; ++sl) re += __ldg(q + sl * slot_stride + (size_t)i0 * F);
-        } else {
-            const int o = i0 * D - i0 * (i0 + 1) / 2 + (j0 - i0 - 1);
-            for (int sl = 0; sl < n_slot; ++sl) {
-                re += __ldg(q + sl * slot_stride + (size_t)(D + 2 * o) * F);
-                im += __ldg(q + sl * slot_stride + (size_t)(D + 2 * o + 1) * F);
-            }
-        }
-        re *= inv_T;
-        im *= inv_T;
-        M[l * P + j] = mk((double)re, (double)(l <= j ? im : -im));
-    }
-}
-
-__device__ __forceinline__ int cta_of_tile_dev(long long i, long long total, int nb) {
-    int b = (int)((i * nb) / total);
-    if (b >= nb) b = nb - 1;
-    while (b + 1 < nb && total * (b + 1) / nb <= i) ++b;
-    while (b > 0 && total * b / nb > i) --b;
-    return b;
-}
-
-template <int D, bool PART>
 __global__ void __launch_bounds__(SolveGeom<D>::THREADS) mwf_solve_kernel(SolveArgs a) {
     using SG = SolveGeom<D>;
     constexpr int P = SG::P, G = SG::G;
@@ -413,27 +318,8 @@ __global__ void __launch_bounds__(SolveGeom<D>::THREADS) mwf_solve_kernel(SolveA
     cd* V = Lm + SG::MAT;                                                      // eigenvectors
     const bool act = l < D;
 
-    if (PART) {
-        const int g = idx / a.F, f = idx % a.F;
-        const long long total = (long long)(a.n_mat / a.F) * a.tiles_per_grp;
-        const int b_first = cta_of_tile_dev((long long)g * a.tiles_per_grp, total, a.n_cta);
-        const int n_slot = cta_of_tile_dev((long long)(g + 1) * a.tiles_per_grp - 1, total, a.n_cta) - b_first + 1;
-        const size_t slot_stride = (size_t)2 * D * D * a.F;
-        const float* q = a.part + (size_t)g * a.slots_per_grp * slot_stride + f;
-        g_load_part<D>(q, n_slot, slot_stride, a.F, a.inv_T, S, l);
-        g_load_part<D>(q + (size_t)D * D * a.F, n_slot, slot_stride, a.F, a.inv_T, Lm, l);
-        if (a.Rss && live && act) {   // optionally also materialise the matrices (API output of the fused op)
-            float2* Rs = const_cast<float2*>(a.Rss) + (size_t)idx * D * D;
-            float2* Rn = const_cast<float2*>(a.Rnn) + (size_t)idx * D * D;
-            for (int j = 0; j < D; ++j) {
-                Rs[l * D + j] = make_float2((float)S[l * P + j].x, (float)S[l * P + j].y);
-                Rn[l * D + j] = make_float2((float)Lm[l * P + j].x, (float)Lm[l * P + j].y);
-            }
-        }
-    } else {
-        g_load_herm<D>(a.Rss + (size_t)idx * D * D, S, l);
-        g_load_herm<D>(a.Rnn + (size_t)idx * D * D, Lm, l);
-    }
+    g_load_herm<D>(a.Rss + (size_t)idx * D * D, S, l);
+    g_load_herm<D>(a.Rnn + (size_t)idx * D * D, Lm, l);
     __syncwarp(gm);
     // first row of Rnn (for conj((Rnn q)[0])) and the traces, before the matrices are overwritten
     const cd n0 = act ? Lm[0 * P + l] : mk(0.0, 0.0);
@@ -581,7 +467,7 @@ template <int D>
 static cudaError_t launch_d(const SolveArgs& a, cudaStream_t st) {
     using SG = SolveGeom<D>;
     const int blocks = (a.n_mat + SG::MPB - 1) / SG::MPB;
-    auto kern = mwf_solve_kernel<D, false>;
+    auto kern = mwf_solve_kernel<D>;
     if (SG::SMEM > 48 * 1024) {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SG::SMEM);
         if (e != cudaSuccess) return e;
@@ -595,7 +481,7 @@ cudaError_t launch_mwf_solve_small(const SolveArgs& a, cudaStream_t st);   // so
 cudaError_t launch_mwf_solve(const SolveArgs& a, cudaStream_t st) {
     if (a.n_mat <= 0) return cudaSuccess;
     if (a.D <= 4) return launch_mwf_solve_small(a, st);
-    if (a.part != nullptr) return cudaErrorInvalidValue;
+    if (a.part != nullptr) return cudaErrorInvalidValue;   // only the D <= 4 solver reads the partial sums
     switch (a.D) {
         case 5: return launch_d<5>(a, st);
         case 6: return launch_d<6>(a, st);

@@ -246,14 +246,6 @@ DISCO_DEV void load_part(const float* __restrict__ q, int n_slot, size_t slot_st
     }
 }
 
-__device__ __forceinline__ int cta_of_tile_dev(long long i, long long total, int nb) {
-    int b = (int)((i * nb) / total);
-    if (b >= nb) b = nb - 1;
-    while (b + 1 < nb && total * (b + 1) / nb <= i) ++b;
-    while (b > 0 && total * b / nb > i) --b;
-    return b;
-}
-
 template <int D, int MINB, bool PART>
 __global__ void __launch_bounds__(64, MINB) mwf_solve_kernel(SolveArgs a) {
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;
@@ -267,8 +259,7 @@ __global__ void __launch_bounds__(64, MINB) mwf_solve_kernel(SolveArgs a) {
         const int n_grp = a.n_mat / (a.F * n_set);
         const int set = idx / (n_grp * a.F), g = (idx / a.F) % n_grp, f = idx % a.F;
         const long long total = (long long)n_grp * a.tiles_per_grp;
-        const int b_first = cta_of_tile_dev((long long)g * a.tiles_per_grp, total, a.n_cta);
-        const int n_slot = cta_of_tile_dev((long long)(g + 1) * a.tiles_per_grp - 1, total, a.n_cta) - b_first + 1;
+        const int n_slot = seg_slots(g, a.tiles_per_grp, total, a.n_cta).count();
         const size_t slot_stride = (size_t)n_set * 2 * D * D * a.F;
         const float* q = a.part + (size_t)g * a.slots_per_grp * slot_stride + (size_t)set * 2 * D * D * a.F + f;
         load_part<D>(q, n_slot, slot_stride, a.F, a.inv_T, S);

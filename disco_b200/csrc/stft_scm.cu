@@ -37,38 +37,6 @@
 #include "fft_reg.cuh"
 #include "kernels.h"
 
-// tuning knobs (scripts/build_variants.py builds alternatives for A/B runs; DESIGN.md 4.1 has the H100 results)
-#ifndef DISCO_SS_PF
-#define DISCO_SS_PF 0          // tiles ahead of the TMA load that the loader prefetches into L2 (0 = off)
-#endif
-#ifndef DISCO_SS_FW
-#define DISCO_SS_FW 8          // FFT warps for up to 4 microphones (8 jobs per tile: 8 or 4)
-#endif
-#ifndef DISCO_SS_FG
-#define DISCO_SS_FG 1          // FFT warp groups working on alternate (smaller) tiles; 2 * FG pipeline stages
-#endif
-#ifndef DISCO_SS_FFTHI
-#define DISCO_SS_FFTHI 0       // 1: FFT warps get the highest warp indices (issue priority), SCM warps the lower ones
-#endif
-// setmaxnreg budgets per thread of the roles (kernels that reallocate registers only).  The sm_90a build of every
-// 256- and 512-point variant is free of local-memory spills with these (ptxas -v); the loader needs 32 for the two
-// Nyquist pair slots of 7-8 microphones, and the FFT warps 104-112 for a 512-point transform.
-#ifndef DISCO_SS_RLEAD
-#define DISCO_SS_RLEAD 32      // loader warpgroup
-#endif
-#ifndef DISCO_SS_RFFT
-#define DISCO_SS_RFFT 256      // cap of the FFT warps' budget, which is what the other roles leave
-#endif
-#ifndef DISCO_SS_RSCM_WIDE
-#define DISCO_SS_RSCM_WIDE 184 // SCM warps, 5..8 microphones
-#endif
-#ifndef DISCO_SS_RSCM_FW4
-#define DISCO_SS_RSCM_FW4 152  // SCM warps, up to 4 microphones next to 4 FFT warps
-#endif
-#ifndef DISCO_SS_RSCM_FW8
-#define DISCO_SS_RSCM_FW8 120  // SCM warps, up to 4 microphones next to 8 FFT warps
-#endif
-
 namespace disco {
 
 template <int N, int C, int NM = 1>
@@ -78,11 +46,8 @@ struct StftCfg {
     static constexpr int HALF = N / 2;             // hop (50 % overlap)
     static constexpr int F = N / 2 + 1;            // bins
     static constexpr bool WIDE = C > 4;            // 128 accumulators per bin
-    // FFT warp groups: group g transforms tiles it = g (mod FG); the tile shrinks with FG so that the shared-memory
-    // budget is unchanged while the pipeline gets 2 * FG stages (deeper input prefetch, finer hand-over to the SCM warps)
-    static constexpr int FG = (!WIDE && N == 512) ? DISCO_SS_FG : 1;
-    static constexpr int NSTG = 2 * FG;            // pipeline stages (samples and spectra)
-    static constexpr int JOBS = 8 / FG;            // jobs per tile
+    static constexpr int NSTG = 2;                 // pipeline stages (samples and spectra)
+    static constexpr int JOBS = 8;                 // jobs per tile
     static constexpr int ITEMS = JOBS * NB;        // (frame, channel-pair) transforms per tile
     static constexpr int P = (C + 1) / 2;          // channel pairs per frame
     static constexpr int TT = ITEMS / P;           // frames per tile
@@ -90,11 +55,10 @@ struct StftCfg {
     // two-mask runs (64) need more registers than an even split of the register file gives them.
     static constexpr bool REALLOC = (N == 512) || (WIDE && N == 256);
     // with two masks the SCM warps carry as much work as the FFT warps, and four FFT warps running two jobs each
-    // per tile leave the SCM warps 152 registers; with one mask eight FFT warps are faster (H100 A/B of the ss_
-    // variants of scripts/build_variants.py: 218-220 us against 223-226 with four, 64 x 4 mics x 10 s)
-    static constexpr int FFT_WARPS = (WIDE && N == 512) ? 4 : (WIDE ? 8 : ((NM == 2 && N == 512) ? 4 : DISCO_SS_FW));
-    static constexpr int FWG = FFT_WARPS / FG;     // FFT warps per group
-    static constexpr int JPW = JOBS / FWG;         // jobs per FFT warp and tile
+    // per tile leave the SCM warps 152 registers; with one mask eight FFT warps are faster (H100 A/B:
+    // 218-220 us against 223-226 with four, 64 x 4 mics x 10 s; DESIGN.md 4.1)
+    static constexpr int FFT_WARPS = (N == 512 && (WIDE || NM == 2)) ? 4 : 8;
+    static constexpr int JPW = JOBS / FFT_WARPS;   // jobs per FFT warp and tile
     static constexpr int ROWP = 1056 / NB;         // spectrum row pitch (complex): a job = 32 x 33 scratch
     static constexpr int SCM_WARPS = N / 64;       // bins 0 .. N/2-1, one per thread
     static constexpr int LEAD_WARPS = REALLOC ? 4 : 1;   // warp 0 = loader; 1..3 idle (warpgroup padding)
@@ -104,23 +68,24 @@ struct StftCfg {
     static constexpr int SAMP = C * (TT + 1) * HALF;   // floats per sample stage
     // registers per thread at launch: each of the 4 SM sub-partitions holds 16384 registers and ceil(WARPS/4) warps
     static constexpr int REG_LAUNCH = 16384 / ((WARPS + 3) / 4) / 32 / 8 * 8;
-    // REALLOC only: fixed budgets for the loader and the SCM warps; the FFT warps get what is left of the CTA's
-    // allocation (a multiple of 8), capped at DISCO_SS_RFFT
-    static constexpr int REG_LEAD = DISCO_SS_RLEAD;
-    static constexpr int REG_SCM = WIDE ? DISCO_SS_RSCM_WIDE : (FFT_WARPS == 4 ? DISCO_SS_RSCM_FW4 : DISCO_SS_RSCM_FW8);
+    // REALLOC only: setmaxnreg budgets per thread of the roles.  The sm_90a build of every 256- and 512-point
+    // variant is free of local-memory spills with these (ptxas -v); the loader needs 32 for the two Nyquist pair
+    // slots of 7-8 microphones, and the FFT warps 104-112 for a 512-point transform.  The loader warpgroup and the
+    // SCM warps (5..8 microphones / up to 4 next to 4 FFT warps / up to 4 next to 8 FFT warps) get fixed budgets;
+    // the FFT warps get what is left of the CTA's allocation (a multiple of 8), capped at 256.
+    static constexpr int REG_LEAD = 32;
+    static constexpr int REG_SCM = WIDE ? 184 : (FFT_WARPS == 4 ? 152 : 120);
+    static constexpr int REG_FFT_CAP = 256;
     static constexpr int REG_ALLOC = (REG_LAUNCH > 255 ? 255 : REG_LAUNCH) * THREADS;
     static constexpr int REG_FFT_LEFT = (REG_ALLOC - 128 * REG_LEAD - 32 * SCM_WARPS * REG_SCM) / (32 * FFT_WARPS) / 8 * 8;
-    static constexpr int REG_FFT = REG_FFT_LEFT < DISCO_SS_RFFT ? REG_FFT_LEFT : DISCO_SS_RFFT;
+    static constexpr int REG_FFT = REG_FFT_LEFT < REG_FFT_CAP ? REG_FFT_LEFT : REG_FFT_CAP;
     static constexpr int REG_SUM = 128 * REG_LEAD + 32 * FFT_WARPS * REG_FFT + 32 * SCM_WARPS * REG_SCM;
     static_assert(!REALLOC || (REG_LEAD >= 24 && REG_FFT >= 24), "setmaxnreg budgets start at 24");
     static_assert(!REALLOC || REG_SUM <= (REG_LAUNCH > 255 ? 255 : REG_LAUNCH) * THREADS,
                   "register budgets exceed the CTA's allocation");
 };
 
-int stft_tile_frames(int n_fft, int C) {
-    const int fg = (C <= 4 && n_fft == 512) ? DISCO_SS_FG : 1;
-    return ((8 / fg) * (32 / (n_fft / 32))) / ((C + 1) / 2);
-}
+int stft_tile_frames(int n_fft, int C) { return (8 * (32 / (n_fft / 32))) / ((C + 1) / 2); }
 
 template <int N, int C>
 __host__ __device__ inline size_t smem_bytes() {
@@ -130,15 +95,6 @@ __host__ __device__ inline size_t smem_bytes() {
 }
 
 __device__ __forceinline__ long long range_lo(long long total, int b, int nb) { return total * b / nb; }
-
-// first CTA whose tile range contains tile i
-__host__ __device__ __forceinline__ int cta_of_tile(long long i, long long total, int nb) {
-    int b = (int)((i * nb) / total);
-    if (b >= nb) b = nb - 1;
-    while (b + 1 < nb && total * (b + 1) / nb <= i) ++b;
-    while (b > 0 && total * b / nb > i) --b;
-    return b;
-}
 
 // Warpgroup register reallocation: grow (inc) or shrink (dec) relative to the launch allocation; the PTX
 // rules make the wrong direction undefined behaviour (an illegal-instruction fault).
@@ -237,8 +193,8 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM>::THREADS, 1) stft_scm_kernel
     float2* tw = reinterpret_cast<float2*>(samp + NSTG * SAMP);          // [RA][32]
     uint64_t* bars = reinterpret_cast<uint64_t*>(tw + N);
     uint64_t* samp_full = bars;               // [NSTG]  loader -> FFT   (1 arrival + TMA bytes)
-    uint64_t* samp_empty = bars + NSTG;       // [NSTG]  FFT -> loader   (FWG arrivals)
-    uint64_t* spec_full = bars + 2 * NSTG;    // [NSTG]  FFT -> SCM      (FWG arrivals)
+    uint64_t* samp_empty = bars + NSTG;       // [NSTG]  FFT -> loader   (FFT_WARPS arrivals)
+    uint64_t* spec_full = bars + 2 * NSTG;    // [NSTG]  FFT -> SCM      (FFT_WARPS arrivals)
     uint64_t* spec_empty = bars + 3 * NSTG;   // [NSTG]  SCM -> FFT      (SCM_WARPS + 1 arrivals)
     float* nyq = reinterpret_cast<float*>(bars + 32);   // [TT * C <= 64] Nyquist-bin values of the current tile
     static_assert(4 * NSTG <= 32, "barrier area");
@@ -256,8 +212,8 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM>::THREADS, 1) stft_scm_kernel
     if (tid == 0) {
         for (int s = 0; s < NSTG; ++s) {
             mbar_init(&samp_full[s], 1);
-            mbar_init(&samp_empty[s], G::FWG);
-            mbar_init(&spec_full[s], G::FWG);
+            mbar_init(&samp_empty[s], G::FFT_WARPS);
+            mbar_init(&spec_full[s], G::FFT_WARPS);
             mbar_init(&spec_empty[s], G::SCM_WARPS + 1);
         }
         fence_mbar_init();
@@ -269,18 +225,15 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM>::THREADS, 1) stft_scm_kernel
         grp = (int)(i / tiles_per_grp);
         t0 = (int)(i % tiles_per_grp) * TT;
     };
-    auto seg_slot = [&](int grp) {
-        return blockIdx.x - cta_of_tile((long long)grp * tiles_per_grp, total, gridDim.x);
-    };
+    auto seg_slot = [&](int grp) { return blockIdx.x - seg_slots(grp, tiles_per_grp, total, gridDim.x).first; };
     auto mask_at = [&](int q, int grp, int t, int f) {
         const float* m = q == 0 ? p.mask : p.mask2;
         return p.mask_ft ? m[((size_t)grp * F + f) * T + t] : m[((size_t)grp * T + t) * F + f];
     };
 
-    // role layout: lead warp(s) first; then FFT and SCM warps in the order DISCO_SS_FFTHI selects (the warp
-    // scheduler favours higher warp indices among ready warps, and the FFT warps are the critical path)
-    constexpr int FFT_WARP0 = G::LEAD_WARPS + (DISCO_SS_FFTHI ? G::SCM_WARPS : 0);
-    constexpr int SCM_WARP0 = G::LEAD_WARPS + (DISCO_SS_FFTHI ? 0 : G::FFT_WARPS);
+    // role layout: lead warp(s), then the FFT warps, then the SCM warps
+    constexpr int FFT_WARP0 = G::LEAD_WARPS;
+    constexpr int SCM_WARP0 = G::LEAD_WARPS + G::FFT_WARPS;
     const bool is_fft = warp >= FFT_WARP0 && warp < FFT_WARP0 + G::FFT_WARPS;
     if (warp < G::LEAD_WARPS) {
         if (G::REALLOC) set_maxnreg<G::REG_LEAD, G::REG_LAUNCH>();
@@ -341,25 +294,10 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM>::THREADS, 1) stft_scm_kernel
 #pragma unroll
                 for (int u = 0; u < NSLOT; ++u) as[q][u] = an[q][u] = 0.f;
         };
-        // L2 prefetch of the in-range samples of tile `it` (DISCO_SS_PF tiles ahead of its TMA load)
-        auto prefetch_tile = [&](int it) {
-            if (!p.use_tma || it >= n_it) return;
-            int grp, t0;
-            tile_of(it, grp, t0);
-            const int nfr = min(TT, T - t0), c_valid = min(C, p.n_sig - grp * C);
-            const int s0 = t0 * H - H, cnt = (nfr + 1) * H;
-            const int k_lo = max(0, -s0), k_hi = min(cnt, L - s0);
-            if (k_hi > k_lo && lane < c_valid)
-                tma_prefetch_l2(p.x + ((size_t)grp * C + lane) * L + s0 + k_lo, (uint32_t)((k_hi - k_lo) * sizeof(float)));
-        };
         nyq_reset();
-        if (DISCO_SS_PF > 0) {
-            for (int i = NSTG - 1; i < NSTG - 1 + DISCO_SS_PF; ++i) prefetch_tile(i);
-        }
         for (int i = 0; i < NSTG - 1; ++i)
             if (i < n_it) load_tile(i);
         for (int it = 0; it < n_it; ++it) {
-            if (DISCO_SS_PF > 0) prefetch_tile(it + NSTG - 1 + DISCO_SS_PF);
             if (it + NSTG - 1 < n_it) load_tile(it + NSTG - 1);
             int grp, t0;
             tile_of(it, grp, t0);
@@ -429,14 +367,17 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM>::THREADS, 1) stft_scm_kernel
     } else if (is_fft) {
         if (G::REALLOC) set_maxnreg<G::REG_FFT, G::REG_LAUNCH>();
         // =========================================================== FFT warps
-        const int wf = warp - FFT_WARP0, fgrp = wf / G::FWG, w = wf % G::FWG;   // group, index within the group
+        // f0 = wf / FFT_WARPS is always 0 and w = wf % FFT_WARPS always wf.  They stay runtime values on purpose: with
+        // a constant first tile and a constant barrier id nvcc schedules the FFT loop differently, and the cfg2 / cfg3
+        // steps ran 0.4 % / 0.3 % slower (stft_scm<512,4,1> 1 %) on an H100 SXM (700 W)
+        const int wf = warp - FFT_WARP0, f0 = wf / G::FFT_WARPS, w = wf % G::FFT_WARPS;
         constexpr bool WINREG = (RA <= 16);
         float win[WINREG ? RA : 1];   // window for n = lane + 32 j (pre-scaled by 1/2 for the two-for-one split)
         if (WINREG) {
 #pragma unroll
             for (int j = 0; j < RA; ++j) win[j] = p.window[lane + 32 * j];
         }
-        for (int it = fgrp; it < n_it; it += G::FG) {
+        for (int it = f0; it < n_it; ++it) {
             int grp, t0;
             tile_of(it, grp, t0);
             const int nfr = min(TT, T - t0), s = it % NSTG, c_valid = min(C, p.n_sig - grp * C);
@@ -452,10 +393,10 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM>::THREADS, 1) stft_scm_kernel
                 if (n_fill > 0) {   // CTA-uniform: cooperative scalar fill (reflect padding) by the FFT warps
                     const float* xg = p.x + (size_t)grp * C * L;
                     float* dst = samp + s * SAMP;
-                    named_bar_sync(1 + fgrp, 32 * G::FWG);        // every FFT warp of the group is done with this stage
+                    named_bar_sync(1 + f0, 32 * G::FFT_WARPS);        // every FFT warp is done with this stage
                     for (int c = 0; c < c_valid; ++c)
 #pragma unroll 4
-                        for (int q = w * 32 + lane; q < n_fill; q += 32 * G::FWG) {
+                        for (int q = w * 32 + lane; q < n_fill; q += 32 * G::FFT_WARPS) {
                             const int k = q < k_lo ? q : q + (k_hi - k_lo);
                             int sidx = s0 + k;               // librosa center=True, pad_mode='reflect'
                             if (sidx < 0) sidx = -sidx;
@@ -464,7 +405,7 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM>::THREADS, 1) stft_scm_kernel
                             if (sidx >= 0 && sidx < L) v = xg[(size_t)c * L + sidx];
                             dst[c * (TT + 1) * H + k] = v;
                         }
-                    named_bar_sync(1 + fgrp, 32 * G::FWG);
+                    named_bar_sync(1 + f0, 32 * G::FFT_WARPS);
                 }
             }
             mbar_wait(&spec_empty[s], ph ^ 1);                // spectrum stage s free (tile it-2 consumed)
@@ -628,8 +569,7 @@ __global__ void __launch_bounds__(288) scm_finalize_kernel(const float* __restri
     constexpr int NA = 2 * C * C;
     const int g = blockIdx.x;
     const long long total = (long long)n_grp * tiles_per_grp;
-    const int b_first = cta_of_tile((long long)g * tiles_per_grp, total, n_cta);
-    const int n_slot = cta_of_tile((long long)(g + 1) * tiles_per_grp - 1, total, n_cta) - b_first + 1;
+    const int n_slot = seg_slots(g, tiles_per_grp, total, n_cta).count();
     const size_t slot_stride = (size_t)n_set * NA * F;
     for (int f = threadIdx.x; f < F; f += blockDim.x) {
         const float* base = part + (size_t)g * slots_per_grp * slot_stride + (size_t)set * NA * F + f;
@@ -663,14 +603,6 @@ __global__ void __launch_bounds__(288) scm_finalize_kernel(const float* __restri
 int stft_tiles_per_grp(int n_fft, int C, int T) {
     const int tt = stft_tile_frames(n_fft, C);
     return (T + tt - 1) / tt;
-}
-
-// Upper bound on the number of CTAs whose tile range intersects one group.
-int stft_slots_per_grp(int n_grp, int tiles_per_grp, int n_cta) {
-    const long long total = (long long)n_grp * tiles_per_grp;
-    const long long min_range = total / n_cta;   // every CTA owns floor or ceil(total / n_cta) tiles
-    if (min_range == 0) return tiles_per_grp + 1;
-    return (int)(tiles_per_grp / min_range) + 2;
 }
 
 bool stft_scm_supported(int n_fft, int C, int n_mask) {
