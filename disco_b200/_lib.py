@@ -29,6 +29,8 @@ SIGNATURES = {
     "disco_stft_scm2_workspace": (c_size_t, [c_int, c_int, c_int, c_int]),
     "disco_stft_scm2": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p,
                                 c_size_t, c_void_p]),
+    "disco_stft_filter_dual": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
+                                       c_int, c_int, c_int, c_void_p]),
     "disco_scm_from_workspace": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                                          c_void_p]),
     "disco_mwf_solve_workspace2": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,

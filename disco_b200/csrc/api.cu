@@ -132,7 +132,7 @@ int stft_common(const float* x, const float* mask, const float* mask2, int mask_
     if (!stft_scm_supported(n_fft, C, n_mask))
         return fail(DISCO_ERR_UNSUPPORTED,
                     "fused STFT+SCM: 1..8 channels per group (1..4 with two masks or n_fft = 1024)");
-    if (!x || !Y) return fail(DISCO_ERR_INVALID, "null pointer");
+    if (!x || (!Y && n_mask != 2)) return fail(DISCO_ERR_INVALID, "null pointer");   // two masks: Y optional
     Tables tb;
     int rc = get_tables(n_fft, &tb);
     if (rc) return rc;
@@ -219,6 +219,42 @@ int disco_stft_scm2(const float* x, const float* mask_a, const float* mask_b, in
     if (n_grp <= 0) return fail(DISCO_ERR_INVALID, "n_grp must be positive");
     return stft_common(x, mask_a, mask_b, mask_layout, Y, nullptr, nullptr, n_grp * C, C, length, n_fft, workspace,
                        workspace_bytes, 2, stream);
+}
+
+int disco_stft_filter_dual(const float* x, const void* W1, const void* W2, void* z, void* zn, void* yf, int ref,
+                           int out_layout, int n_grp, int C, int length, int n_fft, void* stream) {
+    if (!valid_nfft(n_fft)) return fail(DISCO_ERR_INVALID, "n_fft must be 256, 512 or 1024");
+    if (n_grp < 1 || length <= n_fft / 2)
+        return fail(DISCO_ERR_INVALID, "need n_grp > 0 and length > n_fft/2 (reflect padding)");
+    if (!stft_scm_supported(n_fft, C, 2))
+        return fail(DISCO_ERR_UNSUPPORTED, "fused STFT+filter: 1..4 channels per group, n_fft 256 or 512");
+    if (ref < 0 || ref >= C) return fail(DISCO_ERR_INVALID, "ref channel out of range");
+    if (out_layout != DISCO_LAYOUT_TF && out_layout != DISCO_LAYOUT_FT) return fail(DISCO_ERR_INVALID, "bad out_layout");
+    if (!x || !W1 || !W2 || !z || !yf) return fail(DISCO_ERR_INVALID, "null pointer");
+    Tables tb;
+    int rc = get_tables(n_fft, &tb);
+    if (rc) return rc;
+    const int T = disco_n_frames(length, n_fft);
+    StftFilterArgs a;
+    memset(&a, 0, sizeof(a));
+    a.x = x;
+    a.twiddle = tb.twiddle;
+    a.window = tb.win_half;
+    a.n_sig = n_grp * C;
+    a.n_grp = n_grp;
+    a.L = length;
+    a.T = T;
+    a.use_tma = (length % 4 == 0) && ((reinterpret_cast<uintptr_t>(x) & 15) == 0);
+    a.W1 = (const float2*)W1;
+    a.W2 = (const float2*)W2;
+    a.z = (float2*)z;
+    a.zn = (float2*)zn;
+    a.yf = (float2*)yf;
+    a.ref = ref;
+    a.out_ft = (out_layout == DISCO_LAYOUT_FT);
+    const StftPlan pl = plan_stft(n_grp, C, T, n_fft);
+    CU(launch_stft_filter_dual(a, n_fft, C, pl.n_cta, (cudaStream_t)stream), "stft_filter_dual launch");
+    return 0;
 }
 
 int disco_scm_from_workspace(const void* workspace, int n_set, int set, void* Rss, void* Rnn, int n_grp, int C,

@@ -46,6 +46,26 @@ DISCO_DEV float2 cconj(float2 a) { return make_float2(a.x, -a.y); }
 // acc += s * a   (s real)
 DISCO_DEV float2 cfma_r(float s, float2 a, float2 acc) { return ffma2(make_float2(s, s), a, acc); }
 
+// Both filters of a single-node array at one (frame, bin): z = w1^H y, zn = y[ref] - z, yf = w2^H y, for the fused
+// STFT filter pass.  The same helpers on the same operands in the same order as filter_dual_kernel, so the two agree
+// bit for bit (filter_dual.cu keeps its own copy of these lines: calling this reschedules two of its kernels).
+template <int C>
+DISCO_DEV void dual_filter(const float2 (&w1)[C], const float2 (&w2)[C], const float2 (&y)[C], int ref, float2& z,
+                           float2& zn, float2& yf) {
+    z = make_float2(0.f, 0.f);
+    yf = make_float2(0.f, 0.f);
+#pragma unroll
+    for (int c = 0; c < C; ++c) {
+        z = cfma_cj(w1[c], y[c], z);
+        yf = cfma_cj(w2[c], y[c], yf);
+    }
+    float2 r = y[0];
+#pragma unroll
+    for (int c = 1; c < C; ++c)
+        if (c == ref) r = y[c];
+    zn = csub(r, z);
+}
+
 // ---------------------------------------------------------------- shared-memory / TMA plumbing
 DISCO_DEV uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 

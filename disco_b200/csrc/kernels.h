@@ -23,9 +23,23 @@ struct StftArgs {
     int mask_ft;
     int use_tma;
 };
+// The filter pass (launch_stft_filter_dual): z = w1^H y, zn = y[ref] - z, yf = w2^H y of single-node groups.  Its own
+// parameter type, so the parameter block (and with it the machine code) of the other instantiations stays as it is.
+struct StftFilterArgs : StftArgs {
+    const float2* W1;       // [n_grp][F][C]
+    const float2* W2;       // [n_grp][F][C]
+    float2* z;              // [n_grp][T][F] (out_ft = 0) or [n_grp][F][T] (out_ft = 1)
+    float2* zn;             // same layout, or null
+    float2* yf;             // same layout
+    int ref;
+    int out_ft;
+};
 
-// n_mask: 0 plain STFT, 1 STFT + SCMs under `mask`, 2 STFT + SCMs under `mask` and `mask2`
+// n_mask: 0 plain STFT, 1 STFT + SCMs under `mask`, 2 STFT + SCMs under `mask` and `mask2`.
+// Two masks and Y == null: the statistics only, no spectrum is stored.
 cudaError_t launch_stft_scm(const StftArgs& a, int n_fft, int C, int n_cta, int n_mask, cudaStream_t st);
+// STFT + both filters of a single-node array per (frame, bin), Y never stored; the coverage of n_mask = 2
+cudaError_t launch_stft_filter_dual(const StftFilterArgs& a, int n_fft, int C, int n_cta, cudaStream_t st);
 bool stft_scm_supported(int n_fft, int C, int n_mask);
 // matrices of mask set `set` (of n_set) from the segment partial sums
 cudaError_t launch_scm_finalize(const float* part, float2* Rss, float2* Rnn, int n_grp, int slots_per_grp,

@@ -39,7 +39,13 @@
 
 namespace disco {
 
-template <int N, int C, int NM = 1>
+// What the consumer warps write per (frame, bin): the spectrum Y; nothing (NM > 0: the statistics are the only
+// output); or, with NM = 0, the single-node dual filter  z = w1^H y, zn = y[ref] - z, yf = w2^H y  of filter_dual.cu,
+// so that the filter pass transforms the time signals again instead of reading a stored Y back; OUT_FILTER writes the
+// three outputs frame-major ([T][F]), OUT_FILTER_FT in the reference's (F, T) layout.
+enum : int { OUT_Y = 0, OUT_NONE = 1, OUT_FILTER = 2, OUT_FILTER_FT = 3 };
+
+template <int N, int C, int NM = 1, int OUT = OUT_Y>
 struct StftCfg {
     static constexpr int RA = N / 32;              // radix of the per-lane first pass
     static constexpr int NB = 32 / RA;             // transforms per warp job
@@ -73,13 +79,21 @@ struct StftCfg {
     // slots of 7-8 microphones, and the FFT warps 104-112 for a 512-point transform.  The loader warpgroup and the
     // SCM warps (5..8 microphones / up to 4 next to 4 FFT warps / up to 4 next to 8 FFT warps) get fixed budgets;
     // the FFT warps get what is left of the CTA's allocation (a multiple of 8), capped at 256.
-    static constexpr int REG_LEAD = 32;
-    static constexpr int REG_SCM = WIDE ? 184 : (FFT_WARPS == 4 ? 152 : 120);
+    // The filter consumer (OUT_FILTER) holds 2 C filter taps and one frame's C spectra instead of accumulators, and its
+    // loader also applies the Nyquist-bin filters (2 C taps of its own), so the loader gets more and the consumer far
+    // fewer registers; the FFT warps take what is left as always.
+    static constexpr bool FILT = OUT == OUT_FILTER || OUT == OUT_FILTER_FT;
+    static constexpr int REG_LEAD = FILT ? 56 : 32;
+    static constexpr int REG_SCM = FILT ? 80 : WIDE ? 184 : (FFT_WARPS == 4 ? 152 : 120);
     static constexpr int REG_FFT_CAP = 256;
     static constexpr int REG_ALLOC = (REG_LAUNCH > 255 ? 255 : REG_LAUNCH) * THREADS;
     static constexpr int REG_FFT_LEFT = (REG_ALLOC - 128 * REG_LEAD - 32 * SCM_WARPS * REG_SCM) / (32 * FFT_WARPS) / 8 * 8;
     static constexpr int REG_FFT = REG_FFT_LEFT < REG_FFT_CAP ? REG_FFT_LEFT : REG_FFT_CAP;
     static constexpr int REG_SUM = 128 * REG_LEAD + 32 * FFT_WARPS * REG_FFT + 32 * SCM_WARPS * REG_SCM;
+    // OUT_FILTER_FT: per consumer warp one output of 8 frames x its 32 bins, staged for the transposed store (pitch 34:
+    // conflict-free both as rows of 32 bins and as the columns that 8 lanes (frames) x 4 bins read)
+    static constexpr int FT_PITCH = 34;
+    static constexpr int FT_STAGE = OUT == OUT_FILTER_FT ? SCM_WARPS * 8 * FT_PITCH : 0;   // complex
     static_assert(!REALLOC || (REG_LEAD >= 24 && REG_FFT >= 24), "setmaxnreg budgets start at 24");
     static_assert(!REALLOC || REG_SUM <= (REG_LAUNCH > 255 ? 255 : REG_LAUNCH) * THREADS,
                   "register budgets exceed the CTA's allocation");
@@ -87,11 +101,11 @@ struct StftCfg {
 
 int stft_tile_frames(int n_fft, int C) { return (8 * (32 / (n_fft / 32))) / ((C + 1) / 2); }
 
-template <int N, int C>
+template <int N, int C, int OUT = OUT_Y>
 __host__ __device__ inline size_t smem_bytes() {
-    using G = StftCfg<N, C>;
+    using G = StftCfg<N, C, 1, OUT>;
     return G::NSTG * ((size_t)G::SPEC * sizeof(float2) + (size_t)G::SAMP * sizeof(float)) + (size_t)N * sizeof(float2) + 256 +
-           64 * sizeof(float);
+           64 * sizeof(float) + (size_t)G::FT_STAGE * sizeof(float2);
 }
 
 __device__ __forceinline__ long long range_lo(long long total, int b, int nb) { return total * b / nb; }
@@ -174,14 +188,29 @@ struct ScmAcc {
     }
 };
 
-template <int N, int C, int NM>
-__global__ void __launch_bounds__(StftCfg<N, C, NM>::THREADS, 1) stft_scm_kernel(StftArgs p) {
-    using G = StftCfg<N, C, NM>;
+template <int OUT>
+struct StftParam {
+    using type = StftArgs;
+};
+template <>
+struct StftParam<OUT_FILTER> {
+    using type = StftFilterArgs;
+};
+template <>
+struct StftParam<OUT_FILTER_FT> {
+    using type = StftFilterArgs;
+};
+
+template <int N, int C, int NM, int OUT>
+__global__ void __launch_bounds__(StftCfg<N, C, NM, OUT>::THREADS, 1) stft_scm_kernel(typename StftParam<OUT>::type p) {
+    using G = StftCfg<N, C, NM, OUT>;
     constexpr int RA = G::RA, NB = G::NB, H = G::HALF, F = G::F, ROWP = G::ROWP, P = G::P, TT = G::TT;
     constexpr int SAMP = G::SAMP;
     constexpr int NACC = NM * 2 * C * C;
     constexpr int NMX = NM > 0 ? NM : 1;
     constexpr bool SCM = NM > 0;
+    constexpr bool STORE_Y = OUT == OUT_Y, FILT = G::FILT, FT = OUT == OUT_FILTER_FT;
+    static_assert(!FILT || NM == 0, "the filter consumer accumulates no statistics");
     constexpr int MCAP = (G::REALLOC && G::REG_SCM >= 152 && !G::WIDE) ? 16 : 8;     // mask values in flight per thread
     constexpr int MC = (TT * NM <= MCAP) ? TT : ((MCAP / NMX) < TT ? (MCAP / NMX) : TT);   // frames per mask chunk
     constexpr int NCH = (TT + MC - 1) / MC;
@@ -197,6 +226,7 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM>::THREADS, 1) stft_scm_kernel
     uint64_t* spec_full = bars + 2 * NSTG;    // [NSTG]  FFT -> SCM      (FFT_WARPS arrivals)
     uint64_t* spec_empty = bars + 3 * NSTG;   // [NSTG]  SCM -> FFT      (SCM_WARPS + 1 arrivals)
     float* nyq = reinterpret_cast<float*>(bars + 32);   // [TT * C <= 64] Nyquist-bin values of the current tile
+    float2* ft_stage = reinterpret_cast<float2*>(nyq + 64);   // OUT_FILTER_FT: [SCM_WARPS][8][FT_PITCH]
     static_assert(4 * NSTG <= 32, "barrier area");
     static_assert(TT * C <= 64 && TT <= 32, "Nyquist staging");
 
@@ -295,6 +325,9 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM>::THREADS, 1) stft_scm_kernel
                 for (int u = 0; u < NSLOT; ++u) as[q][u] = an[q][u] = 0.f;
         };
         nyq_reset();
+        // filter consumer: the Nyquist-bin taps of the current group, lane <-> frame
+        float2 nw1[FILT ? C : 1], nw2[FILT ? C : 1];
+        int nw_grp = -1;
         for (int i = 0; i < NSTG - 1; ++i)
             if (i < n_it) load_tile(i);
         for (int it = 0; it < n_it; ++it) {
@@ -302,67 +335,97 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM>::THREADS, 1) stft_scm_kernel
             int grp, t0;
             tile_of(it, grp, t0);
             const int nfr = min(TT, T - t0), s = it % NSTG, c_valid = min(C, p.n_sig - grp * C);
-            float mq[NMX];
+            if constexpr (FILT) {
+                if (grp != nw_grp) {   // a CTA's tile range may cross groups
 #pragma unroll
-            for (int q = 0; q < NMX; ++q) mq[q] = (SCM && lane < nfr) ? mask_at(q, grp, t0 + lane, F - 1) : 0.f;
-            mbar_wait(&spec_full[s], (it / NSTG) & 1);
-#pragma unroll
-            for (int r = lane; r < TT * C; r += 32) {
-                const int tl_l = r / C, c_l = r % C;
-                float yv = 0.f;
-                if (tl_l < nfr && c_l < c_valid) {
-                    const float2 z = spec[s * G::SPEC + (size_t)(tl_l * P + c_l / 2) * ROWP + N / 2];
-                    yv = (c_l & 1) ? z.y + z.y : z.x + z.x;
-                    p.Y[(((size_t)grp * C + c_l) * T + t0 + tl_l) * F + (F - 1)] = make_float2(yv, 0.f);
-                }
-                nyq[r] = yv;
-            }
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&spec_empty[s]);
-            if (SCM) {
-#pragma unroll
-                for (int tl = 0; tl < TT; ++tl) {
-                    if (tl < nfr) {   // warp-uniform
-                        float pr[NSLOT];
-#pragma unroll
-                        for (int u = 0; u < NSLOT; ++u)
-                            pr[u] = nyq[tl * C + pi[u]] * nyq[tl * C + pj[u]];
-#pragma unroll
-                        for (int q = 0; q < NM; ++q) {
-                            const float m = __shfl_sync(0xffffffffu, mq[q], tl), om = 1.f - m;
-                            const float a = m * m, b = om * om;
-#pragma unroll
-                            for (int u = 0; u < NSLOT; ++u) {
-                                as[q][u] = fmaf(a, pr[u], as[q][u]);
-                                an[q][u] = fmaf(b, pr[u], an[q][u]);
-                            }
-                        }
+                    for (int c = 0; c < C; ++c) {
+                        nw1[c] = p.W1[((size_t)grp * F + F - 1) * C + c];
+                        nw2[c] = p.W2[((size_t)grp * F + F - 1) * C + c];
                     }
+                    nw_grp = grp;
                 }
-                const bool seg_end = (it + 1 == n_it) || ((lo + it + 1) % tiles_per_grp == 0);
-                if (seg_end) {
-                    float* out = p.part + ((size_t)grp * p.slots_per_grp + seg_slot(grp)) * NACC * F + (F - 1);
+                mbar_wait(&spec_full[s], (it / NSTG) & 1);
+                if (lane < nfr) {
+                    // the Nyquist spectrum is real; it goes through the complex helpers as (yv, 0), the value
+                    // disco_stft stores there, so z, zn, yf match filter_dual on a stored Y bit for bit
+                    float2 y[C];
 #pragma unroll
-                    for (int u = 0; u < NSLOT; ++u) {
-                        const int pp = lane + 32 * u;
-                        if (pp < NP) {
+                    for (int c = 0; c < C; ++c) {
+                        const float2 z = spec[s * G::SPEC + (size_t)(lane * P + c / 2) * ROWP + N / 2];
+                        y[c] = make_float2((c & 1) ? z.y + z.y : z.x + z.x, 0.f);
+                    }
+                    float2 z, zn, yf;
+                    dual_filter<C>(nw1, nw2, y, p.ref, z, zn, yf);
+                    const size_t o = FT ? ((size_t)grp * F + F - 1) * T + t0 + lane : ((size_t)grp * T + t0 + lane) * F + (F - 1);
+                    __stcs(p.z + o, z);
+                    if (p.zn) __stcs(p.zn + o, zn);
+                    __stcs(p.yf + o, yf);
+                }
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&spec_empty[s]);
+            } else {
+                float mq[NMX];
+#pragma unroll
+                for (int q = 0; q < NMX; ++q) mq[q] = (SCM && lane < nfr) ? mask_at(q, grp, t0 + lane, F - 1) : 0.f;
+                mbar_wait(&spec_full[s], (it / NSTG) & 1);
+#pragma unroll
+                for (int r = lane; r < TT * C; r += 32) {
+                    const int tl_l = r / C, c_l = r % C;
+                    float yv = 0.f;
+                    if (tl_l < nfr && c_l < c_valid) {
+                        const float2 z = spec[s * G::SPEC + (size_t)(tl_l * P + c_l / 2) * ROWP + N / 2];
+                        yv = (c_l & 1) ? z.y + z.y : z.x + z.x;
+                        if (STORE_Y) p.Y[(((size_t)grp * C + c_l) * T + t0 + tl_l) * F + (F - 1)] = make_float2(yv, 0.f);
+                    }
+                    nyq[r] = yv;
+                }
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&spec_empty[s]);
+                if (SCM) {
+#pragma unroll
+                    for (int tl = 0; tl < TT; ++tl) {
+                        if (tl < nfr) {   // warp-uniform
+                            float pr[NSLOT];
+#pragma unroll
+                            for (int u = 0; u < NSLOT; ++u)
+                                pr[u] = nyq[tl * C + pi[u]] * nyq[tl * C + pj[u]];
 #pragma unroll
                             for (int q = 0; q < NM; ++q) {
-                                float* os = out + (size_t)(q * 2 * C * C) * F;
-                                float* on = os + (size_t)(C * C) * F;
-                                os[(size_t)row[u] * F] = as[q][u];
-                                on[(size_t)row[u] * F] = an[q][u];
-                                if (pp >= C) {
-                                    os[(size_t)(row[u] + 1) * F] = 0.f;
-                                    on[(size_t)(row[u] + 1) * F] = 0.f;
+                                const float m = __shfl_sync(0xffffffffu, mq[q], tl), om = 1.f - m;
+                                const float a = m * m, b = om * om;
+#pragma unroll
+                                for (int u = 0; u < NSLOT; ++u) {
+                                    as[q][u] = fmaf(a, pr[u], as[q][u]);
+                                    an[q][u] = fmaf(b, pr[u], an[q][u]);
                                 }
                             }
                         }
                     }
-                    nyq_reset();
+                    const bool seg_end = (it + 1 == n_it) || ((lo + it + 1) % tiles_per_grp == 0);
+                    if (seg_end) {
+                        float* out = p.part + ((size_t)grp * p.slots_per_grp + seg_slot(grp)) * NACC * F + (F - 1);
+#pragma unroll
+                        for (int u = 0; u < NSLOT; ++u) {
+                            const int pp = lane + 32 * u;
+                            if (pp < NP) {
+#pragma unroll
+                                for (int q = 0; q < NM; ++q) {
+                                    float* os = out + (size_t)(q * 2 * C * C) * F;
+                                    float* on = os + (size_t)(C * C) * F;
+                                    os[(size_t)row[u] * F] = as[q][u];
+                                    on[(size_t)row[u] * F] = an[q][u];
+                                    if (pp >= C) {
+                                        os[(size_t)(row[u] + 1) * F] = 0.f;
+                                        on[(size_t)(row[u] + 1) * F] = 0.f;
+                                    }
+                                }
+                            }
+                        }
+                        nyq_reset();
+                    }
                 }
+                __syncwarp();   // nyq[] is rewritten by the next tile
             }
-            __syncwarp();   // nyq[] is rewritten by the next tile
         }
     } else if (is_fft) {
         if (G::REALLOC) set_maxnreg<G::REG_FFT, G::REG_LAUNCH>();
@@ -475,6 +538,91 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM>::THREADS, 1) stft_scm_kernel
         // =========================================================== SCM warps: thread <-> bin f
         const int f = (warp - SCM_WARP0) * 32 + lane;   // 0 .. N/2 - 1
         const int fn = (N - f) & (N - 1);
+        if constexpr (FILT) {
+            // =========================================================== filter consumer: thread <-> bin f
+            float2 w1[C], w2[C];
+            int w_grp = -1;
+            for (int it = 0; it < n_it; ++it) {
+                int grp, t0;
+                tile_of(it, grp, t0);
+                const int nfr = min(TT, T - t0), s = it % NSTG;
+                if (grp != w_grp) {   // a CTA's tile range may cross groups
+#pragma unroll
+                    for (int c = 0; c < C; ++c) {
+                        w1[c] = p.W1[((size_t)grp * F + f) * C + c];
+                        w2[c] = p.W2[((size_t)grp * F + f) * C + c];
+                    }
+                    w_grp = grp;
+                }
+                const float2* stage = spec + s * G::SPEC;
+                // un-mix as below and filter frame tl of bin f
+                auto point = [&](int tl, float2& z, float2& zn, float2& yf) {
+                    float2 y[C];
+#pragma unroll
+                    for (int pr = 0; pr < P; ++pr) {
+                        const float2* row = stage + (size_t)(tl * P + pr) * ROWP;
+                        const float2 zf = row[f], zb = row[fn];
+                        y[2 * pr] = fadd2(zf, make_float2(zb.x, -zb.y));
+                        if (2 * pr + 1 < C) y[2 * pr + 1] = fadd2(make_float2(zf.y, -zf.x), make_float2(zb.y, zb.x));
+                    }
+                    dual_filter<C>(w1, w2, y, p.ref, z, zn, yf);
+                };
+                mbar_wait(&spec_full[s], (it / NSTG) & 1);
+                if constexpr (!FT) {
+                    // frame-major rows, coalesced over the bins of a warp
+                    const size_t o = ((size_t)grp * T + t0) * F + f;
+#pragma unroll 8
+                    for (int tl = 0; tl < TT; ++tl) {
+                        if (tl < nfr) {
+                            float2 z, zn, yf;
+                            point(tl, z, zn, yf);
+                            __stcs(p.z + o + (size_t)tl * F, z);
+                            if (p.zn) __stcs(p.zn + o + (size_t)tl * F, zn);
+                            __stcs(p.yf + o + (size_t)tl * F, yf);
+                        }
+                    }
+                } else {
+                    // (F, T) layout: 8 frames at a time, one output after the other through the warp's staging rows,
+                    // then lanes <-> (frame lane % 8, bin lane / 8 + 4 k): 64 contiguous bytes per bin and store
+                    float2* st = ft_stage + (warp - SCM_WARP0) * 8 * G::FT_PITCH;
+                    const int fw = (warp - SCM_WARP0) * 32, jl = lane & 7;
+                    auto flush = [&](float2* out, int c8) {
+                        __syncwarp();
+                        if (c8 + jl < nfr) {
+#pragma unroll
+                            for (int k = 0; k < 8; ++k) {
+                                const int i = (lane >> 3) + 4 * k;
+                                __stcs(out + ((size_t)grp * F + fw + i) * T + t0 + c8 + jl, st[jl * G::FT_PITCH + i]);
+                            }
+                        }
+                        __syncwarp();
+                    };
+#pragma unroll 1
+                    for (int c8 = 0; c8 < nfr; c8 += 8) {
+                        float2 znr[8], yfr[8];
+#pragma unroll
+                        for (int j = 0; j < 8; ++j) {
+                            float2 z = make_float2(0.f, 0.f);
+                            znr[j] = yfr[j] = z;
+                            if (c8 + j < nfr) point(c8 + j, z, znr[j], yfr[j]);
+                            st[j * G::FT_PITCH + lane] = z;
+                        }
+                        flush(p.z, c8);
+                        if (p.zn) {
+#pragma unroll
+                            for (int j = 0; j < 8; ++j) st[j * G::FT_PITCH + lane] = znr[j];
+                            flush(p.zn, c8);
+                        }
+#pragma unroll
+                        for (int j = 0; j < 8; ++j) st[j * G::FT_PITCH + lane] = yfr[j];
+                        flush(p.yf, c8);
+                    }
+                }
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&spec_empty[s]);
+            }
+            return;
+        }
         ScmAcc<C, NM> acc;
         float mk[NMX][MC];
         // masks of chunk `ch` of tile `it` (a chunk past the CTA's last tile loads nothing): one base pointer per
@@ -534,9 +682,11 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM>::THREADS, 1) stft_scm_kernel
                             y[2 * pr] = fadd2(zf, make_float2(zn.x, -zn.y));
                             if (2 * pr + 1 < C) y[2 * pr + 1] = fadd2(make_float2(zf.y, -zf.x), make_float2(zn.y, zn.x));
                         }
+                        if (STORE_Y) {
 #pragma unroll
-                        for (int c = 0; c < C; ++c)
-                            if (full || c < c_valid) __stcs(ybase + c * cstride + tl * F, y[c]);
+                            for (int c = 0; c < C; ++c)
+                                if (full || c < c_valid) __stcs(ybase + c * cstride + tl * F, y[c]);
+                        }
                         if (SCM) {
                             float m[NMX];
 #pragma unroll
@@ -613,11 +763,11 @@ bool stft_scm_supported(int n_fft, int C, int n_mask) {
     return true;
 }
 
-template <int N, int C, int NM>
-static cudaError_t launch_one(const StftArgs& a, int n_cta, cudaStream_t st) {
-    using G = StftCfg<N, C, NM>;
-    auto kern = stft_scm_kernel<N, C, NM>;
-    const size_t smem = smem_bytes<N, C>();
+template <int N, int C, int NM, int OUT = OUT_Y>
+static cudaError_t launch_one(const typename StftParam<OUT>::type& a, int n_cta, cudaStream_t st) {
+    using G = StftCfg<N, C, NM, OUT>;
+    auto kern = stft_scm_kernel<N, C, NM, OUT>;
+    const size_t smem = smem_bytes<N, C, OUT>();
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     if (G::REALLOC) {   // setmaxnreg.inc would wait forever if the launch allocation were smaller than the budgets
@@ -635,7 +785,7 @@ static cudaError_t launch_nm(const StftArgs& a, int nm, int n_cta, cudaStream_t 
     if (nm == 0) return launch_one<N, C, 0>(a, n_cta, st);
     if (nm == 1) return launch_one<N, C, 1>(a, n_cta, st);
     if constexpr (C <= 4 && N <= 512) {
-        if (nm == 2) return launch_one<N, C, 2>(a, n_cta, st);
+        if (nm == 2) return a.Y ? launch_one<N, C, 2>(a, n_cta, st) : launch_one<N, C, 2, OUT_NONE>(a, n_cta, st);
     }
     return cudaErrorInvalidValue;
 }
@@ -669,6 +819,17 @@ cudaError_t launch_stft_scm(const StftArgs& a, int n_fft, int C, int n_cta, int 
         case 1024: return launch_c<1024>(a, C, n_mask, n_cta, st);
         default: return cudaErrorInvalidValue;
     }
+}
+
+cudaError_t launch_stft_filter_dual(const StftFilterArgs& a, int n_fft, int C, int n_cta, cudaStream_t st) {
+    if (!stft_scm_supported(n_fft, C, 2)) return cudaErrorInvalidValue;   // the coverage of the two-mask pass
+#define DISCO_SFD(NN, CC)                                                                                  \
+    if (n_fft == NN && C == CC)                                                                            \
+        return a.out_ft ? launch_one<NN, CC, 0, OUT_FILTER_FT>(a, n_cta, st) : launch_one<NN, CC, 0, OUT_FILTER>(a, n_cta, st);
+    DISCO_SFD(256, 1) DISCO_SFD(256, 2) DISCO_SFD(256, 3) DISCO_SFD(256, 4)
+    DISCO_SFD(512, 1) DISCO_SFD(512, 2) DISCO_SFD(512, 3) DISCO_SFD(512, 4)
+#undef DISCO_SFD
+    return cudaErrorInvalidValue;
 }
 
 cudaError_t launch_scm_finalize(const float* part, float2* Rss, float2* Rnn, int n_grp, int slots_per_grp,

@@ -155,11 +155,12 @@ def stft_scm_supported(n_fft, C, n_mask=1):
 
 
 @_on_device
-def stft_scm2(x, mask_a, mask_b, n_fft=512, mask_layout="TF"):
+def stft_scm2(x, mask_a, mask_b, n_fft=512, mask_layout="TF", want_Y=True):
     """Fused STFT + the masked SCMs under TWO masks in one pass (single-node arrays: step-1 and step-2
     statistics are taken over the same Y, reference tango.py:357-364 and :431-440 with K = 1).
     x [G, C, L], masks [G, T, F] (or [G, F, T]) -> Y [G, C, T, F], workspace (partial sums of both sets,
-    consumed by mwf_solve_workspace2 / scm_from_workspace)."""
+    consumed by mwf_solve_workspace2 / scm_from_workspace).  want_Y=False stores no spectrum and returns
+    (None, workspace); the workspace is the same bit for bit."""
     _need(x, torch.float32, "x")
     _need(mask_a, torch.float32, "mask_a")
     _need(mask_b, torch.float32, "mask_b")
@@ -174,7 +175,7 @@ def stft_scm2(x, mask_a, mask_b, n_fft=512, mask_layout="TF"):
     want = (G, T, F) if lay == TF else (G, F, T)
     if tuple(mask_a.shape) != want or tuple(mask_b.shape) != want:
         raise ValueError("mask shapes %s / %s, expected %s" % (tuple(mask_a.shape), tuple(mask_b.shape), want))
-    Y = torch.empty((G, C, T, F), dtype=torch.complex64, device=x.device)
+    Y = torch.empty((G, C, T, F), dtype=torch.complex64, device=x.device) if want_Y else None
     ws_bytes = lib.disco_stft_scm2_workspace(G, C, L, n_fft)
     ws = torch.empty(max(ws_bytes, 16) // 4, dtype=torch.float32, device=x.device)
     _lib.check(lib.disco_stft_scm2(_ptr(x), _ptr(mask_a), _ptr(mask_b), lay, _ptr(Y), G, C, L, n_fft, _ptr(ws),
@@ -227,6 +228,32 @@ def filter_dual(W1, W2, Y, ref=0, n_fft=512, out_layout="TF", want_zn=True):
     yf = torch.empty_like(z)
     _lib.check(_lib.load().disco_filter_dual(_ptr(W1), _ptr(W2), _ptr(Y), _ptr(z), _ptr(zn), _ptr(yf), int(ref), lay,
                                              G, C, T, n_fft, _stream()))
+    return z, zn, yf
+
+
+@_on_device
+def stft_filter_dual(x, W1, W2, ref=0, n_fft=512, out_layout="TF", want_zn=True):
+    """filter_dual(W1, W2, stft(x)) without the spectrum in memory: the fused STFT kernel transforms the time signals
+    again and applies z = w1^H y, zn = y[ref] - z and yf = w2^H y per (frame, bin).  x [G, C, L] float32, W1, W2
+    [G, F, C] -> z, zn, yf [G, T, F] (or [G, F, T], written in that layout by the kernel)."""
+    _need(x, torch.float32, "x")
+    _need(W1, torch.complex64, "W1")
+    _need(W2, torch.complex64, "W2")
+    if x.dim() != 3:
+        raise ValueError("x must be [groups, channels, samples]")
+    G, C, L = x.shape
+    T, F = n_frames(L, n_fft), n_fft // 2 + 1
+    lib = _lib.load()
+    if not lib.disco_stft_scm_supported(n_fft, C, 2):
+        raise NotImplementedError("fused STFT+filter: %d channels at n_fft=%d" % (C, n_fft))
+    if tuple(W1.shape) != (G, F, C) or tuple(W2.shape) != (G, F, C):
+        raise ValueError("W1 / W2 shape %s / %s, expected %s" % (tuple(W1.shape), tuple(W2.shape), (G, F, C)))
+    lay = _layout(out_layout)
+    z = torch.empty((G, T, F) if lay == TF else (G, F, T), dtype=torch.complex64, device=x.device)
+    zn = torch.empty_like(z) if want_zn else None
+    yf = torch.empty_like(z)
+    _lib.check(lib.disco_stft_filter_dual(_ptr(x), _ptr(W1), _ptr(W2), _ptr(z), _ptr(zn), _ptr(yf), int(ref), lay,
+                                          G, C, L, n_fft, _stream()))
     return z, zn, yf
 
 

@@ -169,11 +169,14 @@ def tango_batched(y, s=None, n=None, masks=None, vads=("irm1", "irm1"), mask_for
     final_layout = False          # z_y / zn / yf already in `out_layout`
     R2 = W2 = yf = None
     if fuse_dual:
-        Y, ws = ops.stft_scm2(y.view(B * K, C, L), mask_z.view(B * K, T, F), mask_w.view(B * K, T, F), n_fft)
-        Y = Y.view(B, K, C, T, F)
+        # Y is never stored: the filter pass transforms y again, which moves half the bytes of reading Y back
+        x = y.view(B * K, C, L)
+        _, ws = ops.stft_scm2(x, mask_z.view(B * K, T, F), mask_w.view(B * K, T, F), n_fft, want_Y=False)
         W12, _ = ops.mwf_solve_workspace2(ws, B * K, C, L, n_fft, mu, filter_type, rank)
         W1, W2 = W12[0].view(B, K, F, C), W12[1].view(B, K, F, C)
-        z_y, zn, yf = ops.filter_dual(W1, W2, Y, ref=ref_mic, n_fft=n_fft, out_layout=out_layout)
+        z_y, zn, yf = ops.stft_filter_dual(x, W12[0], W12[1], ref=ref_mic, n_fft=n_fft, out_layout=out_layout)
+        shape = (B, K) + tuple(z_y.shape[1:])
+        z_y, zn, yf = z_y.view(shape), zn.view(shape), yf.view(shape)
         final_layout = True
     else:
         st1 = tango_step1(y, mask_z, n_fft, mu, filter_type, rank, ref_mic, oracle_sn=osn,

@@ -111,15 +111,27 @@ DISCO_API int disco_stft_scm(const float* x, const float* mask, int mask_layout,
 
 /* ---- fused STFT + the SCMs under TWO masks (single-node arrays, both masks known up front) --------
  * For K = 1 the step-2 statistics (reference tango.py:431-440) are taken over the same Y as the step-1
- * statistics (tango.py:357-364), only under mask_w instead of mask_z.  One pass accumulates both sets, so Y
- * is written once here and read once by disco_filter_dual() -- never re-read for statistics.
+ * statistics (tango.py:357-364), only under mask_w instead of mask_z.  One pass accumulates both sets.
  *   mask_a, mask_b [n_grp] planes in `mask_layout`; C <= 4, n_fft in {256, 512}.
+ *   Y [n_grp][C][T][F] complex64, or NULL: no spectrum is stored (the statistics are the same bit for bit).
+ *   disco_stft_filter_dual() then transforms x again to apply both filters, so Y is never written or read.
  * The four matrix sets stay in `workspace` (disco_stft_scm2_workspace() bytes) as per-segment partial sums:
  * disco_mwf_solve_workspace2() solves both filter sets from them in one launch; disco_scm_from_workspace()
  * materialises the matrices of one set (set 0 = mask_a, 1 = mask_b; n_set = 2 here, 1 after disco_stft_scm). */
 DISCO_API size_t disco_stft_scm2_workspace(int n_grp, int C, int length, int n_fft);
 DISCO_API int disco_stft_scm2(const float* x, const float* mask_a, const float* mask_b, int mask_layout, void* Y,
                     int n_grp, int C, int length, int n_fft, void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---- STFT and both filter-and-sum steps of a single-node array in one pass over the time signals ------
+ * disco_filter_dual(W1, W2, disco_stft(x)) without the spectrum in memory: the STFT of every group is computed
+ * again and z = w1^H y, zn = y[ref] - z, yf = w2^H y are applied per (frame, bin), with the same arithmetic as
+ * disco_filter_dual on the spectrum disco_stft stores (identical results when each group's channels are
+ * transformed together, i.e. disco_stft called per group).  Reads 4 C bytes per sample instead of 8 C per bin.
+ *   x [n_grp][C][length] float32; W1, W2 [n_grp][F][C] complex64;
+ *   z, zn (may be NULL), yf [n_grp] planes in `out_layout` complex64.
+ * C <= 4, n_fft in {256, 512} (disco_stft_scm_supported(n_fft, C, 2)). */
+DISCO_API int disco_stft_filter_dual(const float* x, const void* W1, const void* W2, void* z, void* zn, void* yf,
+                                     int ref, int out_layout, int n_grp, int C, int length, int n_fft, void* stream);
 DISCO_API int disco_scm_from_workspace(const void* workspace, int n_set, int set, void* Rss, void* Rnn, int n_grp,
                              int C, int length, int n_fft, void* stream);
 

@@ -2,7 +2,7 @@
 
     ncu --set full --clock-control none --import-source on -k regex:<kernel> -s 2 -c 1 -o out python scripts/prof_target.py <what>
 
-what: stft_scm2 | stft_scm1 | stft | stft_scm_c8 | stft_scm_c8_256 | filter_dual | masked_scm_zf4 | filter_sum4 | istft |
+what: stft_scm2 | stft_scm2_noY | stft_filter_dual | stft_filter_dual_ft | stft_scm1 | stft | stft_scm_c8 | stft_scm_c8_256 | filter_dual | masked_scm_zf4 | filter_sum4 | istft |
       solve4 | solve8 | tango_mid44 | tango_mid28 | filter_multi44 | masked_scm_zf8
 Shapes = the BASELINE workloads (64 x 4 mics x 10 s; 128 x 8 mics x 10 s; 64 x 4 nodes x 4 mics; 64 x 8 nodes x 2 mics)."""
 import os
@@ -26,11 +26,14 @@ def TF(n_fft):
     return 1 + L // (n_fft // 2), n_fft // 2 + 1
 
 
-if what in ("stft_scm2", "stft_scm1", "stft"):
+if what in ("stft_scm2", "stft_scm2_noY", "stft_scm1", "stft", "stft_filter_dual", "stft_filter_dual_ft"):
     T, F = TF(512)
     x, m, m2 = torch.randn((64, 4, L), generator=g).to(dev), rnd(64, T, F), rnd(64, T, F)
-    fn = {"stft_scm2": lambda: ops.stft_scm2(x, m, m2), "stft_scm1": lambda: ops.stft_scm(x, m, keep_partials=True),
-          "stft": lambda: ops.stft(x)}[what]
+    W1, W2 = cplx(64, F, 4), cplx(64, F, 4)
+    fn = {"stft_scm2": lambda: ops.stft_scm2(x, m, m2), "stft_scm2_noY": lambda: ops.stft_scm2(x, m, m2, want_Y=False),
+          "stft_scm1": lambda: ops.stft_scm(x, m, keep_partials=True), "stft": lambda: ops.stft(x),
+          "stft_filter_dual": lambda: ops.stft_filter_dual(x, W1, W2),
+          "stft_filter_dual_ft": lambda: ops.stft_filter_dual(x, W1, W2, out_layout="FT")}[what]
 elif what in ("stft_scm_c8", "stft_scm_c8_256"):
     n_fft = 256 if what.endswith("256") else 512
     T, F = TF(n_fft)
