@@ -16,6 +16,19 @@ DISCO_DEV float2 ffma2(float2 a, float2 b, float2 c) {
     return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
 
+// ---------------------------------------------------------------- per-bin solve
+// 2^-e for t in [2^e, 2^(e+1)); 1 when t is 0, subnormal, inf or NaN.  The MWF solvers multiply Rss and Rnn by
+// it, with t = max(sum |diag Rss| + sum |diag Rnn|, max |Re, Im of any entry|) (the sum for PSD input; the
+// maximum covers indefinite input such as an Rss with a zero diagonal), so every bin is solved in the same
+// binade whatever the units of the input: the product is exact, every filter they compute is invariant under a
+// common scale, and inputs that differ by a power of two give bit-identical filters.  It also puts the absolute 1e-300 of the Cholesky pivot
+// floor at a fixed distance below the data, which keeps singular bins (Rnn == 0) finite at any input scale.
+DISCO_DEV double solve_scale(double t) {
+    if (!(t >= 2.2250738585072014e-308 && t <= 1.7976931348623157e308)) return 1.0;
+    const int e = ((__double2hiint(t) >> 20) & 0x7ff) - 1023;
+    return __hiloint2double((1023 - e) << 20, 0);
+}
+
 // ---------------------------------------------------------------- complex helpers (float2)
 DISCO_DEV float2 cadd(float2 a, float2 b) { return fadd2(a, b); }
 DISCO_DEV float2 csub(float2 a, float2 b) { return fadd2(a, make_float2(-b.x, -b.y)); }

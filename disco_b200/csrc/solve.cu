@@ -19,8 +19,10 @@
 // matrices live in shared memory (no local-memory traffic), and every O(D) loop of the textbook
 // algorithms (column / row updates of a Jacobi rotation, the columns of a triangular solve, ...)
 // is spread over the group's lanes.  Groups synchronise with __syncwarp(group mask) only.
-// Degenerate bins: a Cholesky pivot below 1e-13 * trace/D is floored there (diagonal loading) so
-// the output stays finite where LAPACK would return inf/NaN eigenvalues.
+// Degenerate bins (DESIGN.md section 2; oracle/solve_f64.py states the policy executably): both matrices are
+// scaled by one exact power of two (common.cuh solve_scale), a Cholesky pivot below 1e-13 * trace/D is floored
+// there with the column below it set to zero, so the output stays finite at any scale where LAPACK would return
+// inf/NaN eigenvalues.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -38,6 +40,18 @@ DISCO_DEV cd operator*(cd a, cd b) { return cd{a.x * b.x - a.y * b.y, a.x * b.y 
 DISCO_DEV cd operator*(double s, cd a) { return cd{s * a.x, s * a.y}; }
 DISCO_DEV cd conj(cd a) { return cd{a.x, -a.y}; }
 DISCO_DEV double norm2(cd a) { return a.x * a.x + a.y * a.y; }
+// 1 / z without forming |z|^2 when that would overflow or underflow (z = mu + l v^H u reaches ~1e300 when
+// Rnn == 0 puts u = Rnn^-1 v at 1e300 v); the plain form otherwise, so ordinary bins keep their bits.
+DISCO_DEV cd crecip(cd z) {
+    const double n2 = norm2(z);
+    if (n2 > 1e-290 && n2 < 1e290) {
+        const double dn = 1.0 / n2;
+        return cd{z.x * dn, -z.y * dn};
+    }
+    const double s = 1.0 / fmax(fabs(z.x), fabs(z.y));
+    const double a = s * z.x, b = s * z.y, dn = s / (a * a + b * b);
+    return cd{a * dn, -b * dn};
+}
 
 constexpr double kEps = 2.220446049250313e-16;  // sys.float_info.epsilon (internal_formulas.py:6)
 constexpr double kEta = 1e6;                    // internal_formulas.py:7
@@ -53,6 +67,11 @@ struct SolveGeom {
     static constexpr int MPB = MPW * WARPS;               // matrices per block
     static constexpr int NROT = (D + 1) / 2;              // rotations per Jacobi round
     static constexpr size_t SMEM = (size_t)MPB * (3 * MAT * sizeof(cd) + NROT * 48);
+    // Where shared memory alone caps residency so low that >= 128 registers per thread would still fit (D = 8 and
+    // D >= 12: 3..7 blocks per SM), the launch bounds tell the compiler so; left to itself it picks ~80 registers
+    // and spills at D = 16.  (228 KB of shared memory per SM, 1 KB reserved per block.)
+    static constexpr int SMEM_BLOCKS = (int)(233472 / (SMEM + 1024));
+    static constexpr int MINB = 65536 / (THREADS * SMEM_BLOCKS) >= 128 ? SMEM_BLOCKS : 0;   // 0: no bound
 };
 
 // group-wide sum over the G lanes of a group (xor butterfly: fixed order, every lane gets the total)
@@ -70,7 +89,11 @@ DISCO_DEV cd gsum(cd v, unsigned gm) {
 }
 
 // In-place lower Cholesky of the Hermitian matrix M (lower triangle used) in shared memory.
-// Lane j computes pivot j, lanes i > j their entry of column j.
+// Lane j computes pivot j, lanes i > j their entry of column j.  A running pivot below `floor_` marks a null
+// direction of M (Rnn == 0, a dead or duplicated microphone, a bin with a single noise frame): the pivot is
+// floored and the column below it set to zero.  Dividing that column by the floored pivot instead would
+// amplify the rounding noise of a numerically singular, slightly indefinite M (float32 statistics) by
+// 1/sqrt(floor) per column, up to inf at D = 16.
 template <int D>
 DISCO_DEV void g_cholesky(cd* M, int l, unsigned gm, double floor_) {
     constexpr int P = SolveGeom<D>::P, G = SolveGeom<D>::G;
@@ -79,9 +102,11 @@ DISCO_DEV void g_cholesky(cd* M, int l, unsigned gm, double floor_) {
         if (l == j) {
             double d = M[j * P + j].x;
             for (int k = 0; k < j; ++k) d -= norm2(M[j * P + k]);
+            const bool null_dir = !(d >= floor_);
             d = fmax(d, floor_);
             inv = rsqrt(d);
             M[j * P + j] = mk(d * inv, 0.0);
+            if (null_dir) inv = 0.0;
         }
         inv = __shfl_sync(gm, inv, j, G);
         if (l > j && l < D) {
@@ -203,22 +228,27 @@ DISCO_DEV void g_jacobi(cd* A, cd* V, Rot* rot, int l, unsigned gm) {
     __syncwarp(gm);
 }
 
-// Principal eigenpair of the Hermitian positive semi-definite matrix A (shared memory, preserved) by
-// repeated squaring: B_0 = A / tr A, B_{k+1} = B_k^2 / tr(B_k^2) converges to v v^H with the eigenvalue
-// ratio raised to the power 2^k, i.e. 10 squarings resolve a 3 % gap to 1e-14 and 24 squarings a
-// 1e-5 gap -- a dozen small matrix products instead of ~50 Jacobi rounds with their float64 special
-// functions.  Rank-1 is detected by ||B||_F^2 = 1 (tr B = 1).  Lane l owns row l.  Returns this
-// lane's component of the unit eigenvector (in *v_out) and the eigenvalue v^H A v.
+// Eigenpair of the LARGEST eigenvalue of the Hermitian matrix A (shared memory, preserved) by repeated squaring:
+// B_0 = A / tr A, B_{k+1} = B_k^2 / tr(B_k^2) converges to v v^H with the eigenvalue ratio raised to the power
+// 2^k, i.e. 10 squarings resolve a 3 % gap to 1e-14 and 24 squarings a 1e-5 gap -- a dozen small matrix products
+// instead of ~50 Jacobi rounds with their float64 special functions.  Rank-1 is detected by ||B||_F^2 = 1
+// (tr B = 1); at most 40 squarings, after which B spans the eigenvectors of (nearly) tied eigenvalues and any of
+// its columns is a valid answer.  Lane l owns row l.  Returns this lane's component of the unit eigenvector (in
+// *v_out) and the eigenvalue v^H A v.
+// Squaring finds the eigenvalue of largest MAGNITUDE.  For a PSD matrix (every bin of an SCM pair) that is the
+// largest one.  An indefinite A (user input such as Rss = Ryy - Rnn) whose most negative eigenvalue dominates, or
+// which has eigenvalues +-rho, ends with a v that is not an eigenvector of a positive eigenvalue:
+// ||A v||^2 != (v^H A v)^2 or v^H A v <= 0.  Then *ok is false and the caller takes the Jacobi path, which picks
+// the largest signed eigenvalue.  A PSD matrix with a positive eigenvalue always passes.  tr A <= 1e-300 (the zero
+// matrix, or an indefinite one with zero or negative trace) also goes to the Jacobi path.
 // Used for the rank-1 GEVD-MWF (the only form Tango calls, tango.py:367, :443); rank > 1 keeps Jacobi.
 template <int D>
-DISCO_DEV double g_top_eigpair(const cd* A, cd* B, int l, unsigned gm, cd* v_out) {
+DISCO_DEV double g_top_eigpair(const cd* A, cd* B, int l, unsigned gm, cd* v_out, bool* ok) {
     constexpr int P = SolveGeom<D>::P, G = SolveGeom<D>::G;
     const bool act = l < D;
     const double tr = gsum<G>(act ? A[l * P + l].x : 0.0, gm);
-    if (!(tr > 1e-300)) {                       // zero matrix: any unit vector, eigenvalue 0
-        *v_out = mk(l == 0 ? 1.0 : 0.0, 0.0);
-        return 0.0;
-    }
+    *ok = false;
+    if (!(tr > 1e-300)) return 0.0;             // group-uniform
     if (act) {
         const double it = 1.0 / tr;
         for (int j = 0; j < D; ++j) B[l * P + j] = it * A[l * P + j];
@@ -285,23 +315,30 @@ DISCO_DEV double g_top_eigpair(const cd* A, cd* B, int l, unsigned gm, cd* v_out
     if (act)
         for (int j = 0; j < D; ++j) av = av + A[l * P + j] * B[j];
     const cd lam = gsum<G>(conj(v) * av, gm);
+    const double av2 = gsum<G>(norm2(av), gm);
+    *ok = lam.x > 0.0 && lam.x * lam.x >= (1.0 - 1e-8) * av2;   // group-uniform
     *v_out = v;
     return lam.x;
 }
 
-// Lane l builds row l of the Hermitian-symmetrised matrix from a complex64 [D][D] array.
+// Lane l builds row l of the Hermitian-symmetrised matrix from a complex64 [D][D] array; returns the largest
+// |Re| or |Im| of that row (0 for idle lanes).
 template <int D>
-DISCO_DEV void g_load_herm(const float2* __restrict__ R, cd* M, int l) {
+DISCO_DEV double g_load_herm(const float2* __restrict__ R, cd* M, int l) {
     constexpr int P = SolveGeom<D>::P;
+    double m = 0.0;
     if (l < D)
         for (int j = 0; j < D; ++j) {
             const float2 a = R[l * D + j], b = R[j * D + l];
-            M[l * P + j] = mk(0.5 * ((double)a.x + (double)b.x), 0.5 * ((double)a.y - (double)b.y));
+            const cd v = mk(0.5 * ((double)a.x + (double)b.x), 0.5 * ((double)a.y - (double)b.y));
+            M[l * P + j] = v;
+            m = fmax(m, fmax(fabs(v.x), fabs(v.y)));
         }
+    return m;
 }
 
 template <int D>
-__global__ void __launch_bounds__(SolveGeom<D>::THREADS) mwf_solve_kernel(SolveArgs a) {
+__global__ void __launch_bounds__(SolveGeom<D>::THREADS, SolveGeom<D>::MINB) mwf_solve_kernel(SolveArgs a) {
     using SG = SolveGeom<D>;
     constexpr int P = SG::P, G = SG::G;
     extern __shared__ __align__(16) unsigned char solve_smem[];
@@ -318,8 +355,22 @@ __global__ void __launch_bounds__(SolveGeom<D>::THREADS) mwf_solve_kernel(SolveA
     cd* V = Lm + SG::MAT;                                                      // eigenvectors
     const bool act = l < D;
 
-    g_load_herm<D>(a.Rss + (size_t)idx * D * D, S, l);
-    g_load_herm<D>(a.Rnn + (size_t)idx * D * D, Lm, l);
+    double m = g_load_herm<D>(a.Rss + (size_t)idx * D * D, S, l);
+    m = fmax(m, g_load_herm<D>(a.Rnn + (size_t)idx * D * D, Lm, l));
+    {   // one exact power-of-two scale for both matrices (common.cuh solve_scale)
+        double t = act ? fabs(S[l * P + l].x) + fabs(Lm[l * P + l].x) : 0.0;
+#pragma unroll
+        for (int off = G / 2; off >= 1; off >>= 1) {   // one butterfly for the sum and the maximum
+            t += __shfl_xor_sync(gm, t, off, G);
+            m = fmax(m, __shfl_xor_sync(gm, m, off, G));
+        }
+        const double sc = solve_scale(fmax(t, m));
+        if (act)
+            for (int j = 0; j < D; ++j) {
+                S[l * P + j] = sc * S[l * P + j];
+                Lm[l * P + j] = sc * Lm[l * P + j];
+            }
+    }
     __syncwarp(gm);
     // first row of Rnn (for conj((Rnn q)[0])) and the traces, before the matrices are overwritten
     const cd n0 = act ? Lm[0 * P + l] : mk(0.0, 0.0);
@@ -354,30 +405,35 @@ __global__ void __launch_bounds__(SolveGeom<D>::THREADS) mwf_solve_kernel(SolveA
             S[l * P + l].y = 0.0;
         }
         __syncwarp(gm);
+        bool top_ok = false;   // rank 1 by squaring; Jacobi for rank > 1 and for the bins squaring cannot settle
         if (a.rank == 1) {
             // rank-1 GEVD-MWF: only the principal pair is needed
             cd v;
-            const double lam1 = g_top_eigpair<D>(S, V, l, gm, &v);
-            // q = L^-H v : column-oriented back substitution, one broadcast per step
-            cd q = v;
-            for (int i = D - 1; i >= 0; --i) {
-                cd qi = mk(0.0, 0.0);
-                if (l == i) {
-                    q = (1.0 / Lm[i * P + i].x) * q;
-                    qi = q;
+            const double lam1 = g_top_eigpair<D>(S, V, l, gm, &v, &top_ok);
+            if (top_ok) {
+                // q = L^-H v : column-oriented back substitution, one broadcast per step
+                cd q = v;
+                for (int i = D - 1; i >= 0; --i) {
+                    cd qi = mk(0.0, 0.0);
+                    if (l == i) {
+                        q = (1.0 / Lm[i * P + i].x) * q;
+                        qi = q;
+                    }
+                    qi.x = __shfl_sync(gm, qi.x, i, G);
+                    qi.y = __shfl_sync(gm, qi.y, i, G);
+                    if (l < i) q = q - conj(Lm[i * P + l]) * qi;
                 }
-                qi.x = __shfl_sync(gm, qi.x, i, G);
-                qi.y = __shfl_sync(gm, qi.y, i, G);
-                if (l < i) q = q - conj(Lm[i * P + l]) * qi;
+                if (!act) q = mk(0.0, 0.0);
+                const double lam = fmin(fmax(lam1, kEps), kEta);
+                const cd c0 = gsum<G>(n0 * q, gm);            // (Rnn q)[0] = sum_j Rnn[0][j] q[j]
+                const cd qc = q * conj(c0);
+                w = (lam / (lam + a.mu)) * qc;
+                t1 = qc;
             }
-            if (!act) q = mk(0.0, 0.0);
-            const double lam = fmin(fmax(lam1, kEps), kEta);
-            const cd c0 = gsum<G>(n0 * q, gm);            // (Rnn q)[0] = sum_j Rnn[0][j] q[j]
-            const cd qc = q * conj(c0);
-            w = (lam / (lam + a.mu)) * qc;
-            t1 = qc;
-        } else {
-        g_jacobi<D>(S, V, rot, l, gm);
+        }
+        if (!top_ok) {
+            __syncwarp(gm);                      // the squaring's scratch in V is dead
+            g_jacobi<D>(S, V, rot, l, gm);
             if (act) {      // Q = L^-H V : lane = eigenvector (column), back substitution
                 for (int i = D - 1; i >= 0; --i) {
                     cd s = V[i * P + l];
@@ -433,8 +489,7 @@ __global__ void __launch_bounds__(SolveGeom<D>::THREADS) mwf_solve_kernel(SolveA
         const cd ul = act ? u[l] : mk(0.0, 0.0);
         const cd vhu = gsum<G>(conj(vl) * ul, gm);
         const cd den = mk(a.mu + lmax * vhu.x, lmax * vhu.y);   // real for Hermitian Rnn up to rounding
-        const double dn = 1.0 / norm2(den);
-        const cd inv = mk(den.x * dn, -den.y * dn);
+        const cd inv = crecip(den);
         w = ul * ((lmax * conj(V[0 * P + best])) * inv);
     } else {  // ------------------------------------------------------------------------ mwf
         if (act)

@@ -20,6 +20,18 @@ DISCO_DEV cd operator*(cd a, cd b) { return cd{a.x * b.x - a.y * b.y, a.x * b.y 
 DISCO_DEV cd operator*(double s, cd a) { return cd{s * a.x, s * a.y}; }
 DISCO_DEV cd conj(cd a) { return cd{a.x, -a.y}; }
 DISCO_DEV double norm2(cd a) { return a.x * a.x + a.y * a.y; }
+DISCO_DEV double cmaxabs(cd a, cd b) { return fmax(fmax(fabs(a.x), fabs(a.y)), fmax(fabs(b.x), fabs(b.y))); }
+// 1 / z without forming |z|^2 when that would overflow or underflow (see solve.cu crecip)
+DISCO_DEV cd crecip(cd z) {
+    const double n2 = norm2(z);
+    if (n2 > 1e-290 && n2 < 1e290) {
+        const double dn = 1.0 / n2;
+        return cd{z.x * dn, -z.y * dn};
+    }
+    const double s = 1.0 / fmax(fabs(z.x), fabs(z.y));
+    const double a = s * z.x, b = s * z.y, dn = s / (a * a + b * b);
+    return cd{a * dn, -b * dn};
+}
 
 constexpr double kEps = 2.220446049250313e-16;  // sys.float_info.epsilon (internal_formulas.py:6)
 constexpr double kEta = 1e6;                    // internal_formulas.py:7
@@ -32,7 +44,8 @@ struct Ld {
 };
 
 // In-place lower Cholesky of the Hermitian matrix M (uses the lower triangle); returns L in M's
-// lower triangle with real positive diagonal.  Pivots are floored at `floor_`.
+// lower triangle with real positive diagonal.  Pivots are floored at `floor_`, and the column below a floored
+// pivot is set to zero (solve.cu g_cholesky).
 template <int D>
 DISCO_DEV void cholesky(cd (&M)[D][Ld<D>::v], double floor_) {
     constexpr int U = (D <= 4) ? D : 1;   // small matrices: fully unrolled, register resident
@@ -40,13 +53,14 @@ DISCO_DEV void cholesky(cd (&M)[D][Ld<D>::v], double floor_) {
     for (int j = 0; j < D; ++j) {
         double d = M[j][j].x;
         for (int k = 0; k < j; ++k) d -= norm2(M[j][k]);
+        const bool null_dir = !(d >= floor_);
         d = fmax(d, floor_);
-        const double inv = rsqrt(d), l = d * inv;
+        const double inv = rsqrt(d), l = d * inv, sc = null_dir ? 0.0 : inv;
         M[j][j] = mk(l, 0.0);
         for (int i = j + 1; i < D; ++i) {
             cd s = M[i][j];
             for (int k = 0; k < j; ++k) s = s - M[i][k] * conj(M[j][k]);
-            M[i][j] = inv * s;
+            M[i][j] = sc * s;
         }
     }
 }
@@ -127,82 +141,100 @@ DISCO_DEV void jacobi(cd (&A)[D][Ld<D>::v], cd (&V)[D][Ld<D>::v], double (&lam)[
     for (int i = 0; i < D; ++i) lam[i] = A[i][i].x;
 }
 
-// Principal eigenpair of the Hermitian PSD matrix A by repeated squaring (see solve.cu g_top_eigpair):
-// B <- B^2 / tr(B^2) until ||B||_F^2 = 1 (rank one).  Fully unrolled: B and its square live in
-// registers.  v receives the unit eigenvector, the return value is v^H A v.
+// Eigenpair of the LARGEST eigenvalue of the Hermitian matrix A by repeated squaring (see solve.cu g_top_eigpair):
+// B <- B^2 / tr(B^2) until ||B||_F^2 = 1 (rank one).  Fully unrolled: B and its square live in registers.
+// v receives the unit eigenvector, the return value is v^H A v.  When v is not an eigenvector of a positive
+// eigenvalue (indefinite A, see solve.cu), the squaring is repeated on A - shift I with shift = -1.5 D max |A_ij|
+// below the smallest eigenvalue: that matrix is PSD with the same top eigenvector.  (The cooperative solver takes
+// its Jacobi path instead; a second squaring run there costs registers and spills.)
 template <int D>
 DISCO_DEV double top_eigpair(const cd (&A)[D][Ld<D>::v], cd (&v)[D]) {
-    double tr = 0.0;
+    double tr = 0.0, amax = 0.0;
 #pragma unroll
     for (int i = 0; i < D; ++i) tr += A[i][i].x;
-    if (!(tr > 1e-300)) {
+#pragma unroll
+    for (int i = 0; i < D; ++i)
+#pragma unroll
+        for (int j = 0; j < D; ++j) amax = fmax(amax, fmax(fabs(A[i][j].x), fabs(A[i][j].y)));
+    if (!(amax > 1e-300)) {
 #pragma unroll
         for (int i = 0; i < D; ++i) v[i] = mk(i == 0 ? 1.0 : 0.0, 0.0);
         return 0.0;
     }
-    cd B[D][D];
-    {
-        const double it = 1.0 / tr;
-#pragma unroll
-        for (int i = 0; i < D; ++i)
-#pragma unroll
-            for (int j = 0; j < D; ++j) B[i][j] = it * A[i][j];
-    }
+    double shift = 0.0, nrm = (tr >= 0.5 * amax) ? tr : amax, lam = 0.0;   // tr A >= max |A_ij| for PSD A
 #pragma unroll 1
-    for (int iter = 0; iter < 40; ++iter) {
-        cd C[D][D];
-        double trc = 0.0, fr2 = 0.0;
+    for (int pass = 0; pass < 2; ++pass) {
+        cd B[D][D];
+        {
+            const double it = 1.0 / nrm;
 #pragma unroll
-        for (int i = 0; i < D; ++i)
+            for (int i = 0; i < D; ++i)
 #pragma unroll
-            for (int j = i; j < D; ++j) {           // Hermitian: upper triangle only
-                cd c = B[i][0] * B[0][j];
+                for (int j = 0; j < D; ++j) B[i][j] = it * A[i][j];
 #pragma unroll
-                for (int k = 1; k < D; ++k) c = c + B[i][k] * B[k][j];
-                C[i][j] = c;
-                if (i == j) {
-                    trc += c.x;
-                    fr2 += c.x * c.x;
-                } else {
-                    fr2 += 2.0 * norm2(c);
+            for (int i = 0; i < D; ++i) B[i][i].x = it * (A[i][i].x - shift);
+        }
+#pragma unroll 1
+        for (int iter = 0; iter < 40; ++iter) {
+            cd C[D][D];
+            double trc = 0.0, fr2 = 0.0;
+#pragma unroll
+            for (int i = 0; i < D; ++i)
+#pragma unroll
+                for (int j = i; j < D; ++j) {           // Hermitian: upper triangle only
+                    cd c = B[i][0] * B[0][j];
+#pragma unroll
+                    for (int k = 1; k < D; ++k) c = c + B[i][k] * B[k][j];
+                    C[i][j] = c;
+                    if (i == j) {
+                        trc += c.x;
+                        fr2 += c.x * c.x;
+                    } else {
+                        fr2 += 2.0 * norm2(c);
+                    }
+                }
+            const double it = 1.0 / trc;
+#pragma unroll
+            for (int i = 0; i < D; ++i) {
+                B[i][i] = mk(it * C[i][i].x, 0.0);
+#pragma unroll
+                for (int j = i + 1; j < D; ++j) {
+                    B[i][j] = it * C[i][j];
+                    B[j][i] = conj(B[i][j]);
                 }
             }
-        const double it = 1.0 / trc;
-#pragma unroll
-        for (int i = 0; i < D; ++i) {
-            B[i][i] = mk(it * C[i][i].x, 0.0);
-#pragma unroll
-            for (int j = i + 1; j < D; ++j) {
-                B[i][j] = it * C[i][j];
-                B[j][i] = conj(B[i][j]);
-            }
+            if (1.0 - fr2 * it * it <= 1e-14) break;
         }
-        if (1.0 - fr2 * it * it <= 1e-14) break;
-    }
-    int jm = 0;
-#pragma unroll
-    for (int j = 1; j < D; ++j)
-        if (B[j][j].x > B[jm][jm].x) jm = j;
-    double nv = 0.0;
-#pragma unroll
-    for (int i = 0; i < D; ++i) {
-        cd c = B[i][0];
+        int jm = 0;
 #pragma unroll
         for (int j = 1; j < D; ++j)
-            if (j == jm) c = B[i][j];
-        v[i] = c;
-        nv += norm2(c);
-    }
-    const double inv = rsqrt(nv);
-    double lam = 0.0;
+            if (B[j][j].x > B[jm][jm].x) jm = j;
+        double nv = 0.0;
 #pragma unroll
-    for (int i = 0; i < D; ++i) v[i] = inv * v[i];
+        for (int i = 0; i < D; ++i) {
+            cd c = B[i][0];
 #pragma unroll
-    for (int i = 0; i < D; ++i) {
-        cd av = A[i][0] * v[0];
+            for (int j = 1; j < D; ++j)
+                if (j == jm) c = B[i][j];
+            v[i] = c;
+            nv += norm2(c);
+        }
+        const double inv = rsqrt(nv);
+        double av2 = 0.0;
+        lam = 0.0;
 #pragma unroll
-        for (int j = 1; j < D; ++j) av = av + A[i][j] * v[j];
-        lam += (conj(v[i]) * av).x;
+        for (int i = 0; i < D; ++i) v[i] = inv * v[i];
+#pragma unroll
+        for (int i = 0; i < D; ++i) {
+            cd av = A[i][0] * v[0];
+#pragma unroll
+            for (int j = 1; j < D; ++j) av = av + A[i][j] * v[j];
+            lam += (conj(v[i]) * av).x;
+            av2 += norm2(av);
+        }
+        if (lam > 0.0 && lam * lam >= (1.0 - 1e-8) * av2) break;   // an eigenvector of a positive eigenvalue
+        shift = -1.5 * D * amax;
+        nrm = tr - D * shift;
     }
     return lam;
 }
@@ -276,6 +308,18 @@ __global__ void __launch_bounds__(64, MINB) mwf_solve_kernel(SolveArgs a) {
     } else {
         load_herm<D>(a.Rss + (size_t)idx * D * D, S);
         load_herm<D>(a.Rnn + (size_t)idx * D * D, Nn);
+    }
+    {   // one exact power-of-two scale for both matrices (common.cuh solve_scale)
+        double t = 0.0, m = 0.0;
+        for (int i = 0; i < D; ++i) t += fabs(S[i][i].x) + fabs(Nn[i][i].x);
+        for (int i = 0; i < D; ++i)
+            for (int j = 0; j < D; ++j) m = fmax(m, cmaxabs(S[i][j], Nn[i][j]));
+        const double sc = solve_scale(fmax(t, m));
+        for (int i = 0; i < D; ++i)
+            for (int j = 0; j < D; ++j) {
+                S[i][j] = sc * S[i][j];
+                Nn[i][j] = sc * Nn[i][j];
+            }
     }
     double trn = 0.0, trs = 0.0;
     for (int i = 0; i < D; ++i) trn += Nn[i][i].x, trs += S[i][i].x;
@@ -380,8 +424,7 @@ __global__ void __launch_bounds__(64, MINB) mwf_solve_kernel(SolveArgs a) {
         for (int i = 0; i < D; ++i) vhu = vhu + conj(V[i][best]) * u[i];
         // w = l u conj(v0) / (mu + l v^H u); the denominator is real for Hermitian Rnn
         const cd den = mk(a.mu + l * vhu.x, l * vhu.y);
-        const double dn = 1.0 / norm2(den);
-        const cd inv = mk(den.x * dn, -den.y * dn);
+        const cd inv = crecip(den);
         const cd sc = (l * conj(V[0][best])) * inv;
         for (int i = 0; i < D; ++i) w[i] = u[i] * sc;
     } else {  // ------------------------------------------------------------------------ mwf

@@ -104,9 +104,10 @@ def stft64(x, n_fft=512, hop=256):
 
 
 def offline_tango(y, s=None, n=None, masks=None, n_fft=512, n_hop=256, mu=1.0,
-                  filter_type="gevd", rank=1, mask_for_z="local", mask_power=1):
+                  filter_type="gevd", rank=1, mask_for_z="local", mask_power=1, solve=solve):
     """Two-step Tango in float64.  y (K,C,L).  Either (s, n) for oracle irm masks or
-    masks=(mask_z (K,F,T), mask_w (K,F,T)).  Returns dict of (K,F,T) arrays."""
+    masks=(mask_z (K,F,T), mask_w (K,F,T)).  `solve(Rss, Rnn, mu, filter_type, rank) -> w` is the per-bin
+    filter (e.g. the solver-policy oracle of oracle/solve_f64.py).  Returns dict of (K,F,T) arrays."""
     y = np.asarray(y)
     K, C, _ = y.shape
     Y = np.array([[stft64(c, n_fft, n_hop) for c in y[k]] for k in range(K)])
