@@ -35,8 +35,8 @@ struct StftFilterArgs : StftArgs {
     int out_ft;
 };
 
-// n_mask: 0 plain STFT, 1 STFT + SCMs under `mask`, 2 STFT + SCMs under `mask` and `mask2`.
-// Two masks and Y == null: the statistics only, no spectrum is stored.
+// n_mask: 0 plain STFT (C <= 4: disco_stft groups its signals by at most 4), 1 STFT + SCMs under `mask`, 2 STFT +
+// SCMs under `mask` and `mask2`.  Two masks and Y == null: the statistics only, no spectrum is stored.
 cudaError_t launch_stft_scm(const StftArgs& a, int n_fft, int C, int n_cta, int n_mask, cudaStream_t st);
 // STFT + both filters of a single-node array per (frame, bin), Y never stored; the coverage of n_mask = 2
 cudaError_t launch_stft_filter_dual(const StftFilterArgs& a, int n_fft, int C, int n_cta, cudaStream_t st);

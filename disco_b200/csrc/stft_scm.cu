@@ -760,6 +760,7 @@ bool stft_scm_supported(int n_fft, int C, int n_mask) {
     if (n_fft != 256 && n_fft != 512 && n_fft != 1024) return false;
     if (C > 4 && (n_mask == 2 || n_fft == 1024)) return false;   // 128 accumulators per bin are the register limit
     if (n_mask == 2 && n_fft == 1024) return false;
+    if (n_mask == 0 && C > 4) return false;   // the plain STFT (disco_stft) groups its signals by at most 4
     return true;
 }
 
@@ -782,7 +783,10 @@ static cudaError_t launch_one(const typename StftParam<OUT>::type& a, int n_cta,
 
 template <int N, int C>
 static cudaError_t launch_nm(const StftArgs& a, int nm, int n_cta, cudaStream_t st) {
-    if (nm == 0) return launch_one<N, C, 0>(a, n_cta, st);
+    // the plain STFT (disco_stft) groups its signals by at most 4, so no group of 5..8 runs without a mask
+    if constexpr (C <= 4) {
+        if (nm == 0) return launch_one<N, C, 0>(a, n_cta, st);
+    }
     if (nm == 1) return launch_one<N, C, 1>(a, n_cta, st);
     if constexpr (C <= 4 && N <= 512) {
         if (nm == 2) return a.Y ? launch_one<N, C, 2>(a, n_cta, st) : launch_one<N, C, 2, OUT_NONE>(a, n_cta, st);
