@@ -129,10 +129,8 @@ def stft_scm(x, mask, n_fft=512, mask_layout="TF", keep_partials=False):
 def mwf_solve_workspace(ws, G, C, L, n_fft=512, mu=1.0, type="gevd", rank=1, want_scm=False):
     """mwf_solve on the SCMs a preceding stft_scm(..., keep_partials=True) left in `ws`.
     Returns W, t1 [G, F, C] (and Rss, Rnn [G, F, C, C] when want_scm)."""
-    if type not in FILTER_TYPES:
-        raise AttributeError("Unknown filter reference")
+    ftype, r = _filter_args(type, rank)
     F = n_fft // 2 + 1
-    r = 0 if rank in ("full", "Full", None) else int(rank)
     W = torch.empty((G, F, C), dtype=torch.complex64, device=ws.device)
     T1 = torch.empty_like(W)
     Rss = Rnn = None
@@ -140,7 +138,7 @@ def mwf_solve_workspace(ws, G, C, L, n_fft=512, mu=1.0, type="gevd", rank=1, wan
         Rss = torch.empty((G, F, C, C), dtype=torch.complex64, device=ws.device)
         Rnn = torch.empty_like(Rss)
     _lib.check(_lib.load().disco_mwf_solve_workspace(_ptr(ws), _ptr(W), _ptr(T1), _ptr(Rss), _ptr(Rnn), G, C, L, n_fft,
-                                                     FILTER_TYPES[type], r, float(mu), _stream()))
+                                                     ftype, r, float(mu), _stream()))
     return (W, T1, Rss, Rnn) if want_scm else (W, T1)
 
 
@@ -197,14 +195,12 @@ def scm_from_workspace(ws, G, C, L, n_fft=512, n_set=1, set=0):
 @_on_device
 def mwf_solve_workspace2(ws, G, C, L, n_fft=512, mu=1.0, type="gevd", rank=1):
     """Both filter sets of a stft_scm2 workspace in one launch: W, t1 [2, G, F, C] (0: mask_a, 1: mask_b)."""
-    if type not in FILTER_TYPES:
-        raise AttributeError("Unknown filter reference")
+    ftype, r = _filter_args(type, rank)
     F = n_fft // 2 + 1
-    r = 0 if rank in ("full", "Full", None) else int(rank)
     W = torch.empty((2, G, F, C), dtype=torch.complex64, device=ws.device)
     T1 = torch.empty_like(W)
     _lib.check(_lib.load().disco_mwf_solve_workspace2(_ptr(ws), _ptr(W), _ptr(T1), G, C, L, n_fft,
-                                                      FILTER_TYPES[type], r, float(mu), _stream()))
+                                                      ftype, r, float(mu), _stream()))
     return W, T1
 
 
@@ -273,24 +269,42 @@ def tf_mask(S, N, type="irm1", bin_thr=0.0):
     return M
 
 
-def _sel(node_sel, K):
-    if node_sel is None:
-        return None, K, K
-    arr = (ctypes.c_int * len(node_sel))(*[int(v) for v in node_sel])
-    return arr, len(node_sel), len(node_sel)
-
-
-def _z_dims(Z, B, T, F, z_layout):
-    """K and the layout flag of the exchanged signals: 'BK' = [B, K, T, F], 'KB' = node-major [K, B, T, F]
-    (what an all-gather over node-owning ranks delivers, disco_b200/dist.py)."""
+def _cat_geometry(y_shape, z_shape=None, node_sel=None, z_layout="BK"):
+    """Launch geometry of the concatenated channels [Y ; z of the other nodes] (CatArgs, csrc/kernels.h), checked
+    here because the library only sees pointers.  y_shape = (B, Ksel, C, T, F); z_shape = (B, K, T, F) with
+    z_layout 'BK', node-major (K, B, T, F) with 'KB' (what an all-gather over node-owning ranks delivers,
+    disco_b200/dist.py), or None: no exchange, every (b, k) is an independent single-node problem.  node_sel: the
+    nodes Y holds (None = all K).  Returns n_utt, K, sel (ctypes int array or None), n_sel, z_layout flag."""
+    B, Ks, C, T, F = y_shape
+    if z_shape is None:
+        return B * Ks, 1, None, 1, 0
     if z_layout not in ("BK", "KB"):
         raise ValueError("z_layout must be 'BK' or 'KB'")
-    _need(Z, torch.complex64, "Z")
-    K = Z.shape[1] if z_layout == "BK" else Z.shape[0]
+    K = z_shape[1 if z_layout == "BK" else 0] if len(z_shape) == 4 else 0
     want = (B, K, T, F) if z_layout == "BK" else (K, B, T, F)
-    if tuple(Z.shape) != want:
-        raise ValueError("Z shape %s, expected %s" % (tuple(Z.shape), want))
-    return K, (0 if z_layout == "BK" else 1)
+    if tuple(z_shape) != want:
+        raise ValueError("Z shape %s, expected %s" % (tuple(z_shape), want))
+    sel, n_sel = None, K
+    if node_sel is not None:
+        sel, n_sel = (ctypes.c_int * len(node_sel))(*[int(v) for v in node_sel]), len(node_sel)
+    if Ks != n_sel:
+        raise ValueError("Y holds %d nodes, selection has %d" % (Ks, n_sel))
+    return B, K, sel, n_sel, (0 if z_layout == "BK" else 1)
+
+
+def _cat_args(Y, Z, node_sel, z_layout="BK"):
+    """_cat_geometry of the tensors Y (complex64, [B, Ksel, C, T, F]) and Z (complex64 or None)."""
+    _need(Y, torch.complex64, "Y")
+    if Z is not None:
+        _need(Z, torch.complex64, "Z")
+    return _cat_geometry(tuple(Y.shape), None if Z is None else tuple(Z.shape), node_sel, z_layout)
+
+
+def _filter_args(type, rank):
+    """Library code of an intern_filter type and the eigenpair count (0 = all, for rank 'full' / 'Full' / None)."""
+    if type not in FILTER_TYPES:
+        raise AttributeError("Unknown filter reference")       # internal_formulas.py:79
+    return FILTER_TYPES[type], 0 if rank in ("full", "Full", None) else int(rank)
 
 
 @_on_device
@@ -298,16 +312,8 @@ def masked_scm(Y, mask, Z=None, n_fft=512, mask_layout="TF", node_sel=None, z_la
     """Y [B, Ksel, C, T, F], Z [B, K, T, F] (or [K, B, T, F] with z_layout='KB') or None (K = 1),
     mask [B, Ksel, T, F] / [B, Ksel, F, T] or None
     -> Rss, Rnn [B, Ksel, F, D, D], D = C + K - 1 (own mics, then z of the other nodes)."""
-    _need(Y, torch.complex64, "Y")
+    n_utt, K, sel, n_sel, zl = _cat_args(Y, Z, node_sel, z_layout)
     B, Ks, C, T, F = Y.shape
-    K, zl = (1, 0) if Z is None else _z_dims(Z, B, T, F, z_layout)
-    n_utt = B
-    if Z is None:            # no exchange: every (b, k) is an independent single-node problem
-        n_utt, sel, n_sel = B * Ks, None, 1
-    else:
-        sel, n_sel, _ = _sel(node_sel, K)
-        if Ks != n_sel:
-            raise ValueError("Y holds %d nodes, selection has %d" % (Ks, n_sel))
     lay = _layout(mask_layout)
     if mask is not None:
         _need(mask, torch.float32, "mask")
@@ -378,14 +384,12 @@ def mwf_solve(Rss, Rnn, mu=1.0, type="gevd", rank=1):
     -> W [..., D], t1 [..., D] complex64.  rank 'full'/'Full'/None -> all eigenpairs."""
     _need(Rss, torch.complex64, "Rss")
     _need(Rnn, torch.complex64, "Rnn")
-    if type not in FILTER_TYPES:
-        raise AttributeError("Unknown filter reference")       # internal_formulas.py:79
+    ftype, r = _filter_args(type, rank)
     D = Rss.shape[-1]
     n_mat = Rss.numel() // (D * D)
-    r = 0 if rank in ("full", "Full", None) else int(rank)
     W = torch.empty(Rss.shape[:-1], dtype=torch.complex64, device=Rss.device)
     T1 = torch.empty_like(W)
-    _lib.check(_lib.load().disco_mwf_solve(_ptr(Rss), _ptr(Rnn), _ptr(W), _ptr(T1), n_mat, D, FILTER_TYPES[type], r,
+    _lib.check(_lib.load().disco_mwf_solve(_ptr(Rss), _ptr(Rnn), _ptr(W), _ptr(T1), n_mat, D, ftype, r,
                                            float(mu), _stream()))
     return W, T1
 
@@ -396,16 +400,8 @@ def filter_sum(W, Y, Z=None, conj=True, ref=None, n_fft=512, out_layout="TF", no
     W [B, Ksel, F, D]; Z [B, K, T, F] (or [K, B, T, F] with z_layout='KB');
     returns out (and resid = x[ref] - out when ref is given), [B, Ksel, T, F] or [.., F, T]."""
     _need(W, torch.complex64, "W")
-    _need(Y, torch.complex64, "Y")
+    n_utt, K, sel, n_sel, zl = _cat_args(Y, Z, node_sel, z_layout)
     B, Ks, C, T, F = Y.shape
-    K, zl = (1, 0) if Z is None else _z_dims(Z, B, T, F, z_layout)
-    n_utt = B
-    if Z is None:
-        n_utt, sel, n_sel = B * Ks, None, 1
-    else:
-        sel, n_sel, _ = _sel(node_sel, K)
-        if Ks != n_sel:
-            raise ValueError("Y holds %d nodes, selection has %d" % (Ks, n_sel))
     D = C + K - 1
     if tuple(W.shape) != (B, Ks, F, D):
         raise ValueError("W shape %s, expected %s" % (tuple(W.shape), (B, Ks, F, D)))
@@ -432,29 +428,16 @@ def istft(Y, length, n_fft=512):
     return x
 
 
-def _cat_dims(Y, Z, node_sel):
-    B, Ks, C, T, F = Y.shape
-    K = 1 if Z is None else Z.shape[1]
-    if Z is None:
-        return B * Ks, None, 1, K, C, T, F
-    _need(Z, torch.complex64, "Z")
-    sel, n_sel, _ = _sel(node_sel, K)
-    if Ks != n_sel:
-        raise ValueError("Y holds %d nodes, selection has %d" % (Ks, n_sel))
-    return B, sel, n_sel, K, C, T, F
-
-
 @_on_device
 def scm_recursive(Y, mask, Z=None, lambda_cor=0.95, block=8, power=2, R0=None, n_fft=512, node_sel=None):
     """Exponentially smoothed SCM pair, R <- lambda R + (1 - lambda) w x x^H per frame (reference
     spatial_correlation_matrix, internal_formulas.py:84-103), sampled after every block of `block` frames.
     Y [B, Ksel, C, T, F], Z [B, K, T, F] or None, mask [B, Ksel, T, F] or None, R0 = (R0ss, R0nn) [B, Ksel, F, D, D]
     -> Rss, Rnn [B, Ksel, J, F, D, D], J = ceil(T / block)."""
-    _need(Y, torch.complex64, "Y")
+    n_utt, K, sel, n_sel, _ = _cat_args(Y, Z, node_sel)
     if mask is not None:
         _need(mask, torch.float32, "mask")
-    n_utt, sel, n_sel, K, C, T, F = _cat_dims(Y, Z, node_sel)
-    B, Ks = Y.shape[:2]
+    B, Ks, C, T, F = Y.shape
     D = C + K - 1
     if mask is not None and tuple(mask.shape) != (B, Ks, T, F):
         raise ValueError("mask shape %s, expected %s" % (tuple(mask.shape), (B, Ks, T, F)))
@@ -479,9 +462,8 @@ def filter_sum_blocks(W, Y, Z=None, block=8, lag=1, conj=True, ref=0, n_fft=512,
     """One filter per block of frames: out[t] = W[t // block - lag]^H x[t] (pass-through of channel `ref` while no
     filter exists yet).  W [B, Ksel, J, F, D] -> out, resid = x[ref] - out, [B, Ksel, T, F]."""
     _need(W, torch.complex64, "W")
-    _need(Y, torch.complex64, "Y")
-    n_utt, sel, n_sel, K, C, T, F = _cat_dims(Y, Z, node_sel)
-    B, Ks = Y.shape[:2]
+    n_utt, K, sel, n_sel, _ = _cat_args(Y, Z, node_sel)
+    B, Ks, C, T, F = Y.shape
     D, J = C + K - 1, (T + block - 1) // block
     if tuple(W.shape) != (B, Ks, J, F, D):
         raise ValueError("W shape %s, expected %s" % (tuple(W.shape), (B, Ks, J, F, D)))

@@ -22,11 +22,6 @@ import torch
 from . import ops
 
 OUTPUT_NAMES = ("yf", "sf", "nf", "z_y", "z_s", "z_n", "zn", "masks_z", "mask_w")
-_KNOWN_MASK_FOR_Z = ("local", "distant", "compressed", "use_oracle_refs", "use_oracle_zs", "previous")
-
-
-def _is_oracle_type(t):
-    return isinstance(t, str) and len(t) == 4 and t[:3] in ("irm", "ibm", "iam") and t[3].isdigit()
 
 
 def _ref_plane(X, ref):
@@ -49,6 +44,109 @@ def _ivad_mask(s_ref, n_fft):
     out = torch.zeros((B, K, T, F), dtype=torch.float32, device=s_ref.device)
     out[:, :, :vad.shape[1], :] = vad.to(torch.float32).view(B, K, -1, 1)
     return out
+
+
+# network masks see windows of 21 frames, hop 1, and predict the middle one (reference tango.py:34-35, 340)
+_DNN_WINDOW = dict(win_len=21, win_hop=1, frame_to_pred="mid")
+
+
+def _mask_kind(vad):
+    """'oracle' ('irmX' / 'ibmX' / 'iamX'), 'ivad' or 'dnn' ('crnn' / 'rnn'), as get_mask tells them apart
+    (tango.py:189-223)."""
+    if isinstance(vad, str) and len(vad) == 4 and vad[:3] in ("irm", "ibm", "iam") and vad[3].isdigit():
+        return "oracle"
+    if vad in ("ivad", "crnn", "rnn"):
+        return "ivad" if vad == "ivad" else "dnn"
+    raise ValueError("Unknown value for `mask_type`")                  # tango.py:223
+
+
+def _z_for_mask(k, K, z_sigs):
+    """The compressed signals that feed node k's step-2 mask estimator, in the order of get_z_for_mask
+    (tango.py:158-186): (signal, node) pairs, signal 0 = z_y and 1 = zn.  'zs_hat' / 'zn_hat' take that signal of
+    every other node; any other z_sigs takes z_y, zn of every other node in turn."""
+    others = [j for j in range(K) if j != k]
+    if z_sigs in ("zs_hat", "zn_hat"):
+        return [(int(z_sigs == "zn_hat"), j) for j in others]
+    return [(t, j) for j in others for t in (0, 1)]
+
+
+def _dnn_masks(mod, Y0, z=None, nodes=None, z_sigs="zs_hat"):
+    """Masks `mod` predicts on the device (tango.py:209-215) from Y0 [B, n, T, F], the mixture spectrum of the
+    microphone each estimator listens to, for the nodes `nodes` of the array (default 0 .. n-1).  With
+    z = (z_y, zn) [B, K, T, F] the estimator of node k also hears _z_for_mask(k, K, z_sigs).  -> [B, n, T, F]."""
+    from . import dnn_mask
+    B, n, T, F = Y0.shape
+    nodes = range(n) if nodes is None else nodes
+    ft = lambda a: a.transpose(-1, -2)                                  # frame-major [T, F] -> (F, T) view
+    out = []
+    for b in range(B):
+        for i, k in enumerate(nodes):
+            zl = None if z is None else [ft(z[t][b, j]) for t, j in _z_for_mask(k, z[0].shape[1], z_sigs)]
+            out.append(dnn_mask.estimate_mask(mod, ft(Y0[b, i]), zl, device=Y0.device, **_DNN_WINDOW))
+    return torch.stack(out).view(B, n, T, F)
+
+
+def _step1_mask(vad, mods, ref_spectra, s_ref, y_ref, n_fft):
+    """Step-1 mask [B, K, T, F] of the reference microphone (tango.py:338-342): an oracle type of its clean
+    spectra ref_spectra() -> (S_ref, N_ref), 'ivad' of its clean signal s_ref [B, K, L], or mods[0] on its mixture
+    spectrum y_ref() [B, K, T, F].  The spectra are callables so that each caller keeps its own STFT grouping
+    (the two-for-one FFT makes a channel's bits depend on its partner signal) and computes only what `vad` needs."""
+    kind = _mask_kind(vad)
+    if kind == "ivad":                                                  # tango.py:216-221
+        return _ivad_mask(s_ref, n_fft)
+    if kind == "dnn":
+        return _dnn_masks(mods[0], y_ref())
+    return ops.tf_mask(*ref_spectra(), vad)
+
+
+def _step2_mask(vads, mods, mask_z, ch0_spectra, s0, n_fft, Y0=None, z=None, nodes=None, z_sigs="zs_hat",
+                ref_mic=0):
+    """Step-2 mask [B, n, T, F] (tango.py:387-394).  mask_z itself for the step-1 oracle kind on the same
+    microphone, or for a network step without a model of its own (mods[1] None, tango.py:388-389); otherwise an
+    oracle type or 'ivad' of microphone 0 (ch0_spectra, s0 as in _step1_mask) or mods[1] on Y0 [B, n, T, F]
+    (microphone 0 of the nodes `nodes`) and the compressed signals z = (z_y, zn) chosen by z_sigs."""
+    if _mask_kind(vads[1]) == "dnn":
+        return mask_z if mods[1] is None else _dnn_masks(mods[1], Y0, z, nodes, z_sigs)
+    if vads[1] == vads[0] and ref_mic == 0:
+        return mask_z
+    return _step1_mask(vads[1], None, ch0_spectra, s0, None, n_fft)
+
+
+def _z_for_stats(mask_for_z, vads, Z, mask_w, Zs, Zn, oracle_refs):
+    """What the other nodes contribute to the step-2 speech / noise statistics (tango.py:396-429): (z_rs, z_rn)
+    [B, K, T, F] from the compressed signals Z, the step-2 masks mask_w, the filtered clean components Zs, Zn and
+    oracle_refs() -> clean spectra of the reference microphones; (None, None) for 'local', where z is masked by
+    the step-2 mask of the node being filtered."""
+    if mask_for_z == "local":
+        return None, None
+    if mask_for_z == "distant":
+        return ops.apply_mask(Z, mask_w, False), ops.apply_mask(Z, mask_w, True)
+    if mask_for_z == "compressed":
+        mc = ops.tf_mask(Zs, Zn, vads[0])
+        return ops.apply_mask(Z, mc, False), ops.apply_mask(Z, mc, True)
+    if mask_for_z == "use_oracle_refs":
+        return oracle_refs()
+    if mask_for_z == "use_oracle_zs":
+        return Zs, Zn
+    if mask_for_z == "use_oracle_sigs":
+        raise NotImplementedError("'use_oracle_sigs' is ill-formed in the reference (tango.py:423-427 "
+                                  "indexes per-channel arrays by node)")
+    return Z, Z              # 'previous' and any other string: unmasked z in both statistics (tango.py:428-429)
+
+
+def _reference_lists(res, names, vads, masks=None):
+    """res[name] [K, ...] NumPy arrays -> the reference's lists of K arrays, one per name.  Like the reference,
+    oracle 'ibmX' masks are bool and 'ivad' masks float64; externally supplied masks stay float32."""
+    out = []
+    for nm in names:
+        arr = res[nm]
+        vad = {"masks_z": vads[0], "mask_w": vads[1]}.get(nm) if masks is None else None
+        if vad is not None and "ibm" in vad:
+            arr = arr.astype(bool)
+        elif vad == "ivad":
+            arr = arr.astype(np.float64)
+        out.append([arr[k] for k in range(len(arr))])
+    return tuple(out)
 
 
 def tango_step1(y, mask_z, n_fft=512, mu=1.0, filter_type="gevd", rank=1, ref_mic=0, oracle_sn=None,
@@ -133,19 +231,11 @@ def tango_batched(y, s=None, n=None, masks=None, vads=("irm1", "irm1"), mask_for
         S, N = ops.stft(s, n_fft), ops.stft(n, n_fft)
     # ---- masks
     if oracle:
-        for v in vads:
-            if not (_is_oracle_type(v) or v == "ivad"):
-                raise ValueError("Unknown value for `mask_type`")      # tango.py:223
-
-        def oracle_mask(kind, ch):
-            if kind == "ivad":                                          # tango.py:216-221
-                return _ivad_mask(s[:, :, ch], n_fft)
-            return ops.tf_mask(_ref_plane(S, ch), _ref_plane(N, ch), kind)
-        mask_z = oracle_mask(vads[0], ref_mic)
-        if vads[1] == vads[0] and ref_mic == 0:
-            mask_w = mask_z
-        else:
-            mask_w = oracle_mask(vads[1], 0)                            # channel 0, tango.py:391
+        if "dnn" in [_mask_kind(v) for v in vads]:
+            raise ValueError("network masks ('crnn' / 'rnn') come in through masks=")
+        spectra = lambda ch: (_ref_plane(S, ch), _ref_plane(N, ch))
+        mask_z = _step1_mask(vads[0], None, lambda: spectra(ref_mic), s[:, :, ref_mic], None, n_fft)
+        mask_w = _step2_mask(vads, None, mask_z, lambda: spectra(0), s[:, :, 0], n_fft, ref_mic=ref_mic)
     else:
         mask_z, mask_w = masks
         if mask_w is None:
@@ -198,24 +288,8 @@ def tango_batched(y, s=None, n=None, masks=None, vads=("irm1", "irm1"), mask_for
     if have_sn and (diagnostics or mask_for_z in ("compressed", "use_oracle_zs")):
         z_s = ops.filter_sum(W1, S, None, conj=True, n_fft=n_fft)
         z_n = ops.filter_sum(W1, N, None, conj=True, n_fft=n_fft)
-    # ---- what the other nodes contribute to the step-2 statistics (tango.py:396-429)
-    z_rs = z_rn = None
-    if mask_for_z == "local":
-        pass
-    elif mask_for_z == "distant":
-        z_rs, z_rn = ops.apply_mask(z_y, mask_w, False), ops.apply_mask(z_y, mask_w, True)
-    elif mask_for_z == "compressed":
-        mc = ops.tf_mask(z_s, z_n, vads[0])
-        z_rs, z_rn = ops.apply_mask(z_y, mc, False), ops.apply_mask(z_y, mc, True)
-    elif mask_for_z == "use_oracle_refs":
-        z_rs, z_rn = _ref_plane(S, ref_mic), _ref_plane(N, ref_mic)
-    elif mask_for_z == "use_oracle_zs":
-        z_rs, z_rn = z_s, z_n
-    elif mask_for_z == "use_oracle_sigs":
-        raise NotImplementedError("'use_oracle_sigs' is ill-formed in the reference (tango.py:423-427 "
-                                  "indexes per-channel arrays by node)")
-    else:   # 'previous' and any other string: unmasked z in both statistics (tango.py:428-429)
-        z_rs = z_rn = z_y
+    z_rs, z_rn = _z_for_stats(mask_for_z, vads, z_y, mask_w, z_s, z_n,
+                              lambda: (_ref_plane(S, ref_mic), _ref_plane(N, ref_mic)))
     # ---- step 2
     ft = ops._layout(out_layout) == ops.FT
     conv = ops.transpose_last2 if ft else (lambda a: a)
@@ -248,13 +322,19 @@ def _to_dev(sig_lists, nodes, device):
     return torch.from_numpy(arr).to(device)[None]          # [1, len(nodes), C, L]
 
 
+def _to_mask(mlist, nodes, device):
+    """(F, T) masks of the nodes `nodes` -> [1, len(nodes), T, F] float32 on the device."""
+    arr = np.stack([np.asarray(mlist[k], dtype=np.float32) for k in nodes])[None]   # [1, n, F, T]
+    return ops.transpose_last2(torch.from_numpy(np.ascontiguousarray(arr)).to(device))
+
+
 def offline_tango(y, s, n, vads="irm1", mods=None, mask_for_z="local", z_sigs="zs_hat", *,
                   n_fft=512, mu=1, filter_type="gevd", rank=1, masks=None, device="cuda"):
     """Drop-in for disco_theque.speech_enhancement.tango.offline_tango (tango.py:252-457).
 
     y, s, n: [node][channel] 1-D float32 signals (ragged channel counts allowed).  Returns the
     reference's 9 lists (length K) of (F, T) arrays: yf, sf, nf, z_y, z_s, z_n, zn (complex64),
-    masks_z, mask_w (float32; bool for 'ibmX' like the reference).
+    masks_z, mask_w (float32; bool for 'ibmX' and float64 for 'ivad' like the reference).
     Keyword-only extensions: n_fft, mu, filter_type, rank (module constants / literals in the
     reference) and masks=(mask_z[K], mask_w[K]) of (F, T) arrays for externally estimated masks.
     DNN mask types ('crnn') run ``mods`` on the device through disco_b200.dnn_mask.
@@ -263,184 +343,79 @@ def offline_tango(y, s, n, vads="irm1", mods=None, mask_for_z="local", z_sigs="z
         raise TypeError("argument of type 'NoneType' is not iterable")   # reference tango.py:343
     if isinstance(vads, str):
         vads = [vads, vads]                                   # get_z_signals.py:279 passes one string
-    K = len(y)
-    chans = [len(y[k]) for k in range(K)]
-    L = len(y[0][0])
-    T, F = ops.n_frames(L, n_fft), n_fft // 2 + 1
-    uniform = len(set(chans)) == 1
-    use_dnn = masks is None and any("rnn" in v for v in vads)
-    if use_dnn and uniform:
-        return _offline_tango_dnn(y, s, n, vads, mods, mask_for_z, z_sigs, n_fft, mu, filter_type, rank,
-                                  torch.device(device))
     dev = torch.device(device)
-
-    def to_mask(mlist, nodes):
-        arr = np.stack([np.asarray(mlist[k], dtype=np.float32) for k in nodes])[None]   # [1, n, F, T]
-        return ops.transpose_last2(torch.from_numpy(np.ascontiguousarray(arr)).to(dev))
-
-    if uniform:
-        nodes = list(range(K))
-        mk = None if masks is None else (to_mask(masks[0], nodes), to_mask(masks[1], nodes))
-        res = tango_batched(_to_dev(y, nodes, dev), _to_dev(s, nodes, dev), _to_dev(n, nodes, dev), masks=mk,
-                            vads=vads, mask_for_z=mask_for_z, n_fft=n_fft, mu=mu, filter_type=filter_type,
-                            rank=rank, out_layout="FT")
-        res = {k: v[0].cpu().numpy() for k, v in res.items()}
-    else:
-        res = _offline_tango_ragged(y, s, n, vads, mask_for_z, n_fft, mu, filter_type, rank, masks, dev, to_mask,
-                                    mods=mods, z_sigs=z_sigs)
-    is_bool = [masks is None and "ibm" in v for v in vads]
-    is_f64 = [masks is None and v == "ivad" for v in vads]       # the reference's VAD masks are float64
-    out = []
-    for nm in OUTPUT_NAMES:
-        arr = res[nm]
-        if nm == "masks_z" and is_bool[0] or nm == "mask_w" and is_bool[1]:
-            arr = arr.astype(bool)
-        if nm == "masks_z" and is_f64[0] or nm == "mask_w" and is_f64[1]:
-            arr = arr.astype(np.float64)
-        out.append([arr[k] for k in range(K)])
-    return tuple(out)
-
-
-def _offline_tango_dnn(y, s, n, vads, mods, mask_for_z, z_sigs, n_fft, mu, filter_type, rank, dev):
-    """vads[i] == 'crnn' (or 'rnn'): masks predicted on the device by mods[i] (tango.py:209-215).
-    Step 1 feeds |Y_ref| alone; step 2 feeds |Y_0| plus the compressed signals of the other nodes chosen by
-    z_sigs (get_z_for_mask, tango.py:158-186); mods[1] is None with vads[1] == 'crnn' reuses the step-1 mask
-    (tango.py:388-389).  Window length / predicted frame are the reference's constants (tango.py:34-35)."""
-    from . import dnn_mask
-    K = len(y)
-    nodes = list(range(K))
+    if len({len(chans) for chans in y}) != 1:
+        res = _offline_tango_ragged(y, s, n, vads, mods, mask_for_z, z_sigs, masks, n_fft, mu, filter_type, rank, dev)
+        return _reference_lists(res, OUTPUT_NAMES, vads, masks)
+    nodes = list(range(len(y)))
     yd, sd, nd = _to_dev(y, nodes, dev), _to_dev(s, nodes, dev), _to_dev(n, nodes, dev)
-    kw = dict(win_len=21, win_hop=1, frame_to_pred="mid", device=dev)
-    spec_ft = lambda a: a.transpose(-1, -2)                         # frame-major [T, F] -> (F, T) view
-
-    def oracle(kind, ch):
-        S, N = ops.stft(sd[:, :, ch].contiguous(), n_fft), ops.stft(nd[:, :, ch].contiguous(), n_fft)
-        return ops.tf_mask(S, N, kind)
-
-    if "rnn" in vads[0]:
-        Yref = ops.stft(yd[:, :, 0].contiguous(), n_fft)            # ref mic 0 (tango.py:338)
-        mask_z = torch.stack([dnn_mask.estimate_mask(mods[0], spec_ft(Yref[0, k]), None, **kw) for k in nodes])[None]
-    else:
-        mask_z = oracle(vads[0], 0)
-
-    def step2_mask(Y, z_y, zn):
-        if "rnn" not in vads[1]:
-            return oracle(vads[1], 0)
-        if mods[1] is None:
-            return mask_z
-        out = []
-        for k in nodes:
-            others = [j for j in nodes if j != k]
-            if z_sigs in ("zs_hat", "zn_hat"):
-                zin = z_y if z_sigs == "zs_hat" else zn
-                zl = [spec_ft(zin[0, j]) for j in others]
-            else:                                                     # interleaved zs_j, zn_j of the other nodes
-                zl = [spec_ft(t[0, j]) for j in others for t in (z_y, zn)]
-            out.append(dnn_mask.estimate_mask(mods[1], spec_ft(Y[0, k, 0]), zl, **kw))
-        return torch.stack(out)[None]
-
-    res = tango_batched(yd, sd, nd, masks=(mask_z, step2_mask), vads=vads, mask_for_z=mask_for_z, n_fft=n_fft,
-                        mu=mu, filter_type=filter_type, rank=rank, out_layout="FT")
-    res = {k: v[0].cpu().numpy() for k, v in res.items()}
-    return tuple([res[nm][k] for k in range(K)] for nm in OUTPUT_NAMES)
+    mk = None
+    if masks is not None:
+        mk = (_to_mask(masks[0], nodes, dev), _to_mask(masks[1], nodes, dev))
+    elif "dnn" in [_mask_kind(v) for v in vads]:
+        # an oracle mask next to a network one is taken from an STFT of microphone 0 alone
+        mic0 = lambda: (ops.stft(sd[:, :, 0].contiguous(), n_fft), ops.stft(nd[:, :, 0].contiguous(), n_fft))
+        mask_z = _step1_mask(vads[0], mods, mic0, sd[:, :, 0], lambda: ops.stft(yd[:, :, 0].contiguous(), n_fft),
+                             n_fft)
+        # the step-2 estimator hears the other nodes' compressed signals: tango_batched calls it after step 1
+        mk = (mask_z, lambda Y, z_y, zn: _step2_mask(vads, mods, mask_z, mic0, sd[:, :, 0], n_fft, Y[:, :, 0],
+                                                     (z_y, zn), z_sigs=z_sigs))
+    res = tango_batched(yd, sd, nd, masks=mk, vads=vads, mask_for_z=mask_for_z, n_fft=n_fft, mu=mu,
+                        filter_type=filter_type, rank=rank, out_layout="FT")
+    return _reference_lists({k: v[0].cpu().numpy() for k, v in res.items()}, OUTPUT_NAMES, vads, masks)
 
 
-def _offline_tango_ragged(y, s, n, vads, mask_for_z, n_fft, mu, filter_type, rank, masks, dev, to_mask,
-                          mods=None, z_sigs="zs_hat"):
+def _offline_tango_ragged(y, s, n, vads, mods, mask_for_z, z_sigs, masks, n_fft, mu, filter_type, rank, dev):
     """Nodes with different microphone counts (reference tango.py:259-260, 284): step 1 and step 2 run
     once per channel count on the nodes that have it; Z (and the signals the other nodes contribute to the
-    step-2 statistics under every `mask_for_z` mode, tango.py:396-429) always hold all K nodes.
-    Masks: oracle types, externally supplied `masks`, or DNN masks (`mods`, tango.py:209-215) -- the estimators only
-    see the reference microphone and the compressed signals, so they do not care about the channel counts."""
-    if mask_for_z == "use_oracle_sigs":
-        raise NotImplementedError("'use_oracle_sigs' is ill-formed in the reference (tango.py:423-427 "
-                                  "indexes per-channel arrays by node)")
+    step-2 statistics under every `mask_for_z` mode, tango.py:396-429) always hold all K nodes.  The mask
+    estimators only see microphone 0 and the compressed signals, so they do not care about the channel counts.
+    Returns the outputs as [K, F, T] NumPy arrays."""
     K = len(y)
-    L = len(y[0][0])
-    T, F = ops.n_frames(L, n_fft), n_fft // 2 + 1
-    dnn = masks is None and any("rnn" in v for v in vads)
-    if dnn:
-        from . import dnn_mask
-        dkw = dict(win_len=21, win_hop=1, frame_to_pred="mid", device=dev)
-    spec_ft = lambda a: a.transpose(-1, -2)
+    T, F = ops.n_frames(len(y[0][0]), n_fft), n_fft // 2 + 1
     groups = {}
     for k in range(K):
         groups.setdefault(len(y[k]), []).append(k)
-    cplx = lambda: torch.empty((1, K, T, F), dtype=torch.complex64, device=dev)
-    Z, Zs, Zn_, ZN, Sref, Nref, Yref = cplx(), cplx(), cplx(), cplx(), cplx(), cplx(), cplx()
+    # all K nodes: Z = z_y, ZN = zn, Zs / Zn = z_s / z_n, Sref / Nref = clean spectra of microphone 0
+    Z, ZN, Zs, Zn, Sref, Nref = (torch.empty((1, K, T, F), dtype=torch.complex64, device=dev) for _ in range(6))
     MZ = torch.empty((1, K, T, F), dtype=torch.float32, device=dev)
     MW = torch.empty_like(MZ)
     use_osn = "use_oracle_" in mask_for_z
-    keep = {}
+    keep = []
     # ---- step 1 per channel count
     for C, nodes in sorted(groups.items()):
         yd, sd, nd = _to_dev(y, nodes, dev), _to_dev(s, nodes, dev), _to_dev(n, nodes, dev)
         S, N = ops.stft(sd, n_fft), ops.stft(nd, n_fft)
         idx = torch.tensor(nodes, device=dev)
         Sref[0, idx], Nref[0, idx] = S[0, :, 0], N[0, :, 0]
-
-        def om(kind):
-            if kind == "ivad":
-                return _ivad_mask(sd[:, :, 0], n_fft)
-            return ops.tf_mask(_ref_plane(S, 0), _ref_plane(N, 0), kind)
         if masks is not None:
-            mz = to_mask(masks[0], nodes)
-        elif "rnn" in vads[0]:
-            Yr = ops.stft(yd[:, :, 0].contiguous(), n_fft)
-            mz = torch.stack([dnn_mask.estimate_mask(mods[0], spec_ft(Yr[0, i]), None, **dkw)
-                              for i in range(len(nodes))])[None]
+            mz = _to_mask(masks[0], nodes, dev)
         else:
-            mz = om(vads[0])
+            mz = _step1_mask(vads[0], mods, lambda: (_ref_plane(S, 0), _ref_plane(N, 0)), sd[:, :, 0],
+                             lambda: ops.stft(yd[:, :, 0].contiguous(), n_fft), n_fft)
         st1 = tango_step1(yd, mz, n_fft, mu, filter_type, rank, 0, oracle_sn=(S, N) if use_osn else None)
         zs = ops.filter_sum(st1["W1"], S, None, conj=True, n_fft=n_fft)
-        zn_ = ops.filter_sum(st1["W1"], N, None, conj=True, n_fft=n_fft)
-        Z[0, idx], Zs[0, idx], Zn_[0, idx], ZN[0, idx] = st1["z_y"][0], zs[0], zn_[0], st1["zn"][0]
-        Yref[0, idx] = st1["Y"][0, :, 0]
+        zn = ops.filter_sum(st1["W1"], N, None, conj=True, n_fft=n_fft)
+        Z[0, idx], Zs[0, idx], Zn[0, idx], ZN[0, idx] = st1["z_y"][0], zs[0], zn[0], st1["zn"][0]
         MZ[0, idx] = mz[0]
-        keep[C] = (nodes, st1["Y"], S, N, om)
-    # ---- step-2 masks (tango.py:387-394)
-    for C, (nodes, Y, S, N, om) in sorted(keep.items()):
-        idx = torch.tensor(nodes, device=dev)
+        keep.append((nodes, idx, st1["Y"], S, N, sd))
+    # ---- step-2 masks, once every node's compressed signals exist
+    for nodes, idx, Y, S, N, sd in keep:
         if masks is not None:
-            MW[0, idx] = to_mask(masks[1], nodes)[0]
-        elif "rnn" in vads[1]:
-            if mods[1] is None:
-                MW[0, idx] = MZ[0, idx]
-            else:
-                for k in nodes:
-                    others = [j for j in range(K) if j != k]
-                    if z_sigs in ("zs_hat", "zn_hat"):
-                        zin = Z if z_sigs == "zs_hat" else ZN
-                        zl = [spec_ft(zin[0, j]) for j in others]
-                    else:
-                        zl = [spec_ft(t[0, j]) for j in others for t in (Z, ZN)]
-                    MW[0, k] = dnn_mask.estimate_mask(mods[1], spec_ft(Yref[0, k]), zl, **dkw)
+            MW[0, idx] = _to_mask(masks[1], nodes, dev)[0]
         else:
-            MW[0, idx] = (MZ[0, idx] if vads[1] == vads[0] else om(vads[1])[0])
-    # ---- what the other nodes contribute to the step-2 statistics (tango.py:396-429)
-    z_rs = z_rn = None
-    if mask_for_z == "distant":
-        z_rs, z_rn = ops.apply_mask(Z, MW, False), ops.apply_mask(Z, MW, True)
-    elif mask_for_z == "compressed":
-        mc = ops.tf_mask(Zs, Zn_, vads[0])
-        z_rs, z_rn = ops.apply_mask(Z, mc, False), ops.apply_mask(Z, mc, True)
-    elif mask_for_z == "use_oracle_refs":
-        z_rs, z_rn = Sref, Nref
-    elif mask_for_z == "use_oracle_zs":
-        z_rs, z_rn = Zs, Zn_
-    elif mask_for_z != "local":              # 'previous' and any other string: unmasked z in both statistics
-        z_rs = z_rn = Z
+            MW[0, idx] = _step2_mask(vads, mods, MZ[:, idx], lambda: (_ref_plane(S, 0), _ref_plane(N, 0)),
+                                     sd[:, :, 0], n_fft, Y[:, :, 0], (Z, ZN), nodes, z_sigs)[0]
+    z_rs, z_rn = _z_for_stats(mask_for_z, vads, Z, MW, Zs, Zn, lambda: (Sref, Nref))
     # ---- step 2 per channel count
     res = {nm: np.empty((K, F, T), np.complex64) for nm in ("yf", "sf", "nf")}
-    for C, (nodes, Y, S, N, om) in sorted(keep.items()):
-        idx = torch.tensor(nodes, device=dev)
-        mw = MW[:, idx].contiguous()
-        yf, W2 = tango_step2(Y, Z, mw, n_fft, mu, filter_type, rank, "FT", node_sel=nodes, z_rs=z_rs, z_rn=z_rn)
+    for nodes, idx, Y, S, N, sd in keep:
+        yf, W2 = tango_step2(Y, Z, MW[:, idx].contiguous(), n_fft, mu, filter_type, rank, "FT", node_sel=nodes,
+                             z_rs=z_rs, z_rn=z_rn)
         sf = ops.filter_sum(W2, S, Zs, conj=True, n_fft=n_fft, out_layout="FT", node_sel=nodes)
-        nf = ops.filter_sum(W2, N, Zn_, conj=True, n_fft=n_fft, out_layout="FT", node_sel=nodes)
-        for i, k in enumerate(nodes):
-            res["yf"][k], res["sf"][k], res["nf"][k] = yf[0, i].cpu().numpy(), sf[0, i].cpu().numpy(), \
-                nf[0, i].cpu().numpy()
+        nf = ops.filter_sum(W2, N, Zn, conj=True, n_fft=n_fft, out_layout="FT", node_sel=nodes)
+        res["yf"][nodes], res["sf"][nodes], res["nf"][nodes] = yf[0].cpu().numpy(), sf[0].cpu().numpy(), \
+            nf[0].cpu().numpy()
     tr = lambda a: ops.transpose_last2(a)[0].cpu().numpy()
-    res.update(z_y=tr(Z), z_s=tr(Zs), z_n=tr(Zn_), zn=tr(ZN), masks_z=tr(MZ), mask_w=tr(MW))
+    res.update(z_y=tr(Z), z_s=tr(Zs), z_n=tr(Zn), zn=tr(ZN), masks_z=tr(MZ), mask_w=tr(MW))
     return res
