@@ -8,7 +8,9 @@ import ctypes
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.path.join(_HERE, "libdisco_b200.so")
+# DISCO_B200_LIB loads another build of the same ABI instead (an instrumented variant, or an older build to compare
+# against); unset, the library built in-tree is used.
+LIB_PATH = os.environ.get("DISCO_B200_LIB") or os.path.join(_HERE, "libdisco_b200.so")
 
 c_int, c_void_p, c_size_t, c_float, c_double = (ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t,
                                                 ctypes.c_float, ctypes.c_double)

@@ -30,15 +30,18 @@ def _deps_mtime():
     return newest
 
 
-def build(verbose=False, force=False):
-    os.makedirs(OBJ, exist_ok=True)
+def build(verbose=False, force=False, defines=(), lib=LIB, obj=OBJ):
+    """defines: extra -D macros (a measurement variant such as DISCO_ROLE_CLOCKS); such a variant goes to its own
+    lib and obj directory so that it never replaces the in-tree library."""
+    os.makedirs(obj, exist_ok=True)
     hdr = _deps_mtime()
     jobs = []
     for src in SOURCES:
         s = os.path.join(CSRC, src)
-        o = os.path.join(OBJ, src.replace(".cu", ".o"))
+        o = os.path.join(obj, src.replace(".cu", ".o"))
         if force or not os.path.exists(o) or os.path.getmtime(o) < max(os.path.getmtime(s), hdr):
-            cmd = [NVCC] + FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-c", s, "-o", o]
+            cmd = ([NVCC] + FLAGS + ["-D" + d for d in defines] + (["-Xptxas", "-v"] if verbose else []) +
+                   ["-c", s, "-o", o])
             jobs.append(cmd)
 
     def run(cmd):
@@ -51,14 +54,14 @@ def build(verbose=False, force=False):
                 sys.stderr.write(" ".join(cmd) + "\n" + r.stdout + r.stderr + "\n")
             if r.returncode != 0:
                 raise RuntimeError("nvcc failed for %s" % cmd[-3])
-    objs = [os.path.join(OBJ, s.replace(".cu", ".o")) for s in SOURCES]
-    if force or jobs or not os.path.exists(LIB):
-        cmd = [NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"]
+    objs = [os.path.join(obj, s.replace(".cu", ".o")) for s in SOURCES]
+    if force or jobs or not os.path.exists(lib):
+        cmd = [NVCC, "-shared", "-o", lib] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             sys.stderr.write(r.stdout + r.stderr)
             raise RuntimeError("link failed")
-    return LIB
+    return lib
 
 
 if __name__ == "__main__":

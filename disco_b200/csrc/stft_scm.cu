@@ -29,6 +29,9 @@
 // For 5..8 microphones the 128 accumulators of a bin need ~184 registers, so the roles are laid out
 // on warpgroup boundaries and the register file is redistributed with setmaxnreg (loader 32, SCM 184,
 // FFT what is left: 112) -- the same mechanism the TMA/wgmma kernels of this architecture use.
+// Two masks at 512 points (3 or 4 microphones): the loader and 7 FFT warps share the first two
+// warpgroups at 104 registers, the 8 SCM warps get 152, and the 8 FFT jobs of a tile are dealt over
+// the 7 FFT warps across the CTA's tile stream (StftCfg::DEAL).
 //
 // A CTA's tile range may cross group boundaries; accumulators are flushed per (group, CTA)
 // segment into a small workspace and reduced in fixed order by scm_finalize_kernel or directly by
@@ -60,14 +63,22 @@ struct StftCfg {
     // Roles on warpgroup boundaries + setmaxnreg: the SCM warps of wide arrays (128 accumulators) and of
     // two-mask runs (64) need more registers than an even split of the register file gives them.
     static constexpr bool REALLOC = (N == 512) || (WIDE && N == 256);
-    // with two masks the SCM warps carry as much work as the FFT warps, and four FFT warps running two jobs each
-    // per tile leave the SCM warps 152 registers; with one mask eight FFT warps are faster (H100 A/B:
-    // 218-220 us against 223-226 with four, 64 x 4 mics x 10 s; DESIGN.md 4.1)
-    static constexpr int FFT_WARPS = (N == 512 && (WIDE || NM == 2)) ? 4 : 8;
-    static constexpr int JPW = JOBS / FFT_WARPS;   // jobs per FFT warp and tile
+    // with one mask eight FFT warps are faster than four (H100 A/B: 218-220 us against 223-226, 64 x 4 mics x 10 s;
+    // DESIGN.md 4.1).  Two masks at 512 points, 3-4 microphones (DEAL): the SCM warps need 152 registers, which
+    // leaves room for 7 FFT warps at 104 only if the three padding warps of the loader's warpgroup become FFT warps;
+    // the 8 jobs of a tile are dealt over them across the tile stream (job j of the CTA -> warp j mod 7), so no warp
+    // runs two jobs of a tile while another idles.  With 4 FFT warps running two jobs each, the role clocks showed
+    // the FFT warps busy 94 % of the time and the SCM warps waiting on spec_full 40 % (DESIGN.md 4.1).
+    // (3-4 microphones only: a tile of 1-2 microphones is 16 frames, so the single-node 2-microphone cfg 1 runs one tile
+    // per CTA, where dealing cannot shorten the FFT path and its step was 4 % slower.  The two-mask kernels of 1-2
+    // microphones keep 4 FFT warps running two jobs each per tile next to SCM warps at 152 registers.)
+    static constexpr bool DEAL = N == 512 && NM == 2 && C >= 3 && !WIDE;
+    static constexpr int FFT_WARPS = DEAL ? 7 : (N == 512 && (WIDE || NM == 2)) ? 4 : 8;
+    static constexpr int JPW = JOBS / FFT_WARPS;   // jobs per FFT warp and tile (without DEAL)
+    static constexpr int FFT_ARRIVALS = DEAL ? JOBS : FFT_WARPS;   // samp_empty / spec_full arrivals per tile
     static constexpr int ROWP = 1056 / NB;         // spectrum row pitch (complex): a job = 32 x 33 scratch
     static constexpr int SCM_WARPS = N / 64;       // bins 0 .. N/2-1, one per thread
-    static constexpr int LEAD_WARPS = REALLOC ? 4 : 1;   // warp 0 = loader; 1..3 idle (warpgroup padding)
+    static constexpr int LEAD_WARPS = (REALLOC && !DEAL) ? 4 : 1;   // warp 0 = loader; 1..3 idle (warpgroup padding)
     static constexpr int WARPS = LEAD_WARPS + FFT_WARPS + SCM_WARPS;
     static constexpr int THREADS = 32 * WARPS;
     static constexpr int SPEC = ITEMS * ROWP;      // complex per spectrum stage
@@ -82,14 +93,20 @@ struct StftCfg {
     // The filter consumer (OUT_FILTER) holds 2 C filter taps and one frame's C spectra instead of accumulators, and its
     // loader also applies the Nyquist-bin filters (2 C taps of its own), so the loader gets more and the consumer far
     // fewer registers; the FFT warps take what is left as always.
+    // DEAL: the loader shares its warpgroup with three FFT warps, so both leading warpgroups get the FFT budget
+    // (2 x 128 x 104 + 256 x 152 = 65 536, all of the launch allocation of 16 warps x 128).
     static constexpr bool FILT = OUT == OUT_FILTER || OUT == OUT_FILTER_FT;
-    static constexpr int REG_LEAD = FILT ? 56 : 32;
-    static constexpr int REG_SCM = FILT ? 80 : WIDE ? 184 : (FFT_WARPS == 4 ? 152 : 120);
+    static constexpr int REG_SCM = FILT ? 80 : WIDE ? 184 : ((N == 512 && NM == 2) ? 152 : 120);
     static constexpr int REG_FFT_CAP = 256;
     static constexpr int REG_ALLOC = (REG_LAUNCH > 255 ? 255 : REG_LAUNCH) * THREADS;
-    static constexpr int REG_FFT_LEFT = (REG_ALLOC - 128 * REG_LEAD - 32 * SCM_WARPS * REG_SCM) / (32 * FFT_WARPS) / 8 * 8;
+    static constexpr int REG_LEAD_OWN = FILT ? 56 : 32;   // the loader warpgroup's budget without DEAL
+    static constexpr int REG_FFT_LEFT =
+        DEAL ? (REG_ALLOC - 32 * SCM_WARPS * REG_SCM) / (32 * (LEAD_WARPS + FFT_WARPS)) / 8 * 8
+             : (REG_ALLOC - 128 * REG_LEAD_OWN - 32 * SCM_WARPS * REG_SCM) / (32 * FFT_WARPS) / 8 * 8;
     static constexpr int REG_FFT = REG_FFT_LEFT < REG_FFT_CAP ? REG_FFT_LEFT : REG_FFT_CAP;
-    static constexpr int REG_SUM = 128 * REG_LEAD + 32 * FFT_WARPS * REG_FFT + 32 * SCM_WARPS * REG_SCM;
+    static constexpr int REG_LEAD = DEAL ? REG_FFT : REG_LEAD_OWN;
+    static constexpr int REG_SUM = DEAL ? 32 * (LEAD_WARPS + FFT_WARPS) * REG_FFT + 32 * SCM_WARPS * REG_SCM
+                                        : 128 * REG_LEAD + 32 * FFT_WARPS * REG_FFT + 32 * SCM_WARPS * REG_SCM;
     // OUT_FILTER_FT: per consumer warp one output of 8 frames x its 32 bins, staged for the transposed store (pitch 34:
     // conflict-free both as rows of 32 bins and as the columns that 8 lanes (frames) x 4 bins read)
     static constexpr int FT_PITCH = 34;
@@ -97,6 +114,12 @@ struct StftCfg {
     static_assert(!REALLOC || (REG_LEAD >= 24 && REG_FFT >= 24), "setmaxnreg budgets start at 24");
     static_assert(!REALLOC || REG_SUM <= (REG_LAUNCH > 255 ? 255 : REG_LAUNCH) * THREADS,
                   "register budgets exceed the CTA's allocation");
+    static_assert(!DEAL || (REALLOC && LEAD_WARPS + FFT_WARPS == 8 && WARPS == 16 && REG_LAUNCH == 128 &&
+                            REG_FFT == 104 && REG_SUM == 65536),
+                  "DEAL: loader + 7 FFT warps fill two warpgroups at 104 registers next to 8 SCM warps at 152");
+    static_assert(DEAL || WIDE || NM != 2 || N != 512 || (FFT_WARPS == 4 && REG_SCM == 152 && REG_FFT == 176),
+                  "two masks, 1-2 microphones at 512 points: 4 FFT warps at 176 registers next to SCM warps at 152");
+    static_assert(!DEAL || JOBS >= FFT_WARPS, "DEAL: every FFT warp must run a job of every tile (the fill barrier)");
 };
 
 int stft_tile_frames(int n_fft, int C) { return (8 * (32 / (n_fft / 32))) / ((C + 1) / 2); }
@@ -188,6 +211,53 @@ struct ScmAcc {
     }
 };
 
+// Per-role cycle accounting, compiled in only with -DDISCO_ROLE_CLOCKS (scripts/role_clocks.py builds that variant
+// into a library of its own).  Lane 0 of every working warp records clock64 cycles spent in each kind of mbarrier
+// wait, its total cycles from the role's start to its end, and the tiles (and, for the FFT warps, jobs) it processed
+// into g_role_clocks[cta][warp][RC_SLOTS] of the last launch; disco_role_clocks copies the buffer out.  Without the
+// switch RoleClocks is empty and wait() is mbar_wait.
+enum : int { RC_SAMP_FULL = 0, RC_SAMP_EMPTY = 1, RC_SPEC_FULL = 2, RC_SPEC_EMPTY = 3 };
+enum : int { RC_ROLE_LOADER = 1, RC_ROLE_FFT = 2, RC_ROLE_SCM = 3 };
+#ifdef DISCO_ROLE_CLOCKS
+// slots: role, tiles, jobs, total cycles, then the wait cycles of samp_full, samp_empty, spec_full, spec_empty
+constexpr int RC_MAX_CTAS = 1024, RC_SLOTS = 8;
+__device__ unsigned long long g_role_clocks[RC_MAX_CTAS * 32 * RC_SLOTS];
+DISCO_DEV long long rc_clock() {
+    long long t;
+    asm volatile("mov.u64 %0, %%clock64;" : "=l"(t)::"memory");
+    return t;
+}
+struct RoleClocks {
+    long long t0, w[4] = {0, 0, 0, 0};
+    int tiles = 0, jobs = 0;
+    DISCO_DEV RoleClocks() : t0(rc_clock()) {}
+    DISCO_DEV void wait(int k, uint64_t* bar, uint32_t parity) {
+        const long long a = rc_clock();
+        mbar_wait(bar, parity);
+        w[k] += rc_clock() - a;
+    }
+    DISCO_DEV void tile() { ++tiles; }
+    DISCO_DEV void job() { ++jobs; }
+    DISCO_DEV void done(int role) {
+        const long long t1 = rc_clock();
+        if ((threadIdx.x & 31) != 0 || blockIdx.x >= RC_MAX_CTAS) return;
+        unsigned long long* o = g_role_clocks + ((size_t)blockIdx.x * 32 + (threadIdx.x >> 5)) * RC_SLOTS;
+        o[0] = role;
+        o[1] = tiles;
+        o[2] = jobs;
+        o[3] = t1 - t0;
+        for (int k = 0; k < 4; ++k) o[4 + k] = w[k];
+    }
+};
+#else
+struct RoleClocks {
+    DISCO_DEV void wait(int, uint64_t* bar, uint32_t parity) { mbar_wait(bar, parity); }
+    DISCO_DEV void tile() {}
+    DISCO_DEV void job() {}
+    DISCO_DEV void done(int) {}
+};
+#endif
+
 template <int OUT>
 struct StftParam {
     using type = StftArgs;
@@ -222,8 +292,8 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM, OUT>::THREADS, 1) stft_scm_k
     float2* tw = reinterpret_cast<float2*>(samp + NSTG * SAMP);          // [RA][32]
     uint64_t* bars = reinterpret_cast<uint64_t*>(tw + N);
     uint64_t* samp_full = bars;               // [NSTG]  loader -> FFT   (1 arrival + TMA bytes)
-    uint64_t* samp_empty = bars + NSTG;       // [NSTG]  FFT -> loader   (FFT_WARPS arrivals)
-    uint64_t* spec_full = bars + 2 * NSTG;    // [NSTG]  FFT -> SCM      (FFT_WARPS arrivals)
+    uint64_t* samp_empty = bars + NSTG;       // [NSTG]  FFT -> loader   (FFT_ARRIVALS: per warp, or per job with DEAL)
+    uint64_t* spec_full = bars + 2 * NSTG;    // [NSTG]  FFT -> SCM      (FFT_ARRIVALS)
     uint64_t* spec_empty = bars + 3 * NSTG;   // [NSTG]  SCM -> FFT      (SCM_WARPS + 1 arrivals)
     float* nyq = reinterpret_cast<float*>(bars + 32);   // [TT * C <= 64] Nyquist-bin values of the current tile
     float2* ft_stage = reinterpret_cast<float2*>(nyq + 64);   // OUT_FILTER_FT: [SCM_WARPS][8][FT_PITCH]
@@ -242,8 +312,8 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM, OUT>::THREADS, 1) stft_scm_k
     if (tid == 0) {
         for (int s = 0; s < NSTG; ++s) {
             mbar_init(&samp_full[s], 1);
-            mbar_init(&samp_empty[s], G::FFT_WARPS);
-            mbar_init(&spec_full[s], G::FFT_WARPS);
+            mbar_init(&samp_empty[s], G::FFT_ARRIVALS);
+            mbar_init(&spec_full[s], G::FFT_ARRIVALS);
             mbar_init(&spec_empty[s], G::SCM_WARPS + 1);
         }
         fence_mbar_init();
@@ -265,15 +335,19 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM, OUT>::THREADS, 1) stft_scm_k
     constexpr int FFT_WARP0 = G::LEAD_WARPS;
     constexpr int SCM_WARP0 = G::LEAD_WARPS + G::FFT_WARPS;
     const bool is_fft = warp >= FFT_WARP0 && warp < FFT_WARP0 + G::FFT_WARPS;
+    if constexpr (G::DEAL) {   // loader + FFT warps: one budget over both leading warpgroups
+        if (warp < SCM_WARP0) set_maxnreg<G::REG_FFT, G::REG_LAUNCH>();
+    }
     if (warp < G::LEAD_WARPS) {
-        if (G::REALLOC) set_maxnreg<G::REG_LEAD, G::REG_LAUNCH>();
+        if (G::REALLOC && !G::DEAL) set_maxnreg<G::REG_LEAD, G::REG_LAUNCH>();
         if (warp != 0) return;
         // =========================================================== LOADER (+ Nyquist bin)
+        RoleClocks rc;
         auto load_tile = [&](int it) {
             int grp, t0;
             tile_of(it, grp, t0);
             const int nfr = min(TT, T - t0), s = it % NSTG, c_valid = min(C, p.n_sig - grp * C);
-            mbar_wait(&samp_empty[s], ((it / NSTG) & 1) ^ 1);
+            rc.wait(RC_SAMP_EMPTY, &samp_empty[s], ((it / NSTG) & 1) ^ 1);
             const float* xg = p.x + (size_t)grp * C * L;
             float* dst = samp + s * SAMP;
             const int s0 = t0 * H - H;
@@ -344,7 +418,7 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM, OUT>::THREADS, 1) stft_scm_k
                     }
                     nw_grp = grp;
                 }
-                mbar_wait(&spec_full[s], (it / NSTG) & 1);
+                rc.wait(RC_SPEC_FULL, &spec_full[s], (it / NSTG) & 1);
                 if (lane < nfr) {
                     // the Nyquist spectrum is real; it goes through the complex helpers as (yv, 0), the value
                     // disco_stft stores there, so z, zn, yf match filter_dual on a stored Y bit for bit
@@ -367,7 +441,7 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM, OUT>::THREADS, 1) stft_scm_k
                 float mq[NMX];
 #pragma unroll
                 for (int q = 0; q < NMX; ++q) mq[q] = (SCM && lane < nfr) ? mask_at(q, grp, t0 + lane, F - 1) : 0.f;
-                mbar_wait(&spec_full[s], (it / NSTG) & 1);
+                rc.wait(RC_SPEC_FULL, &spec_full[s], (it / NSTG) & 1);
 #pragma unroll
                 for (int r = lane; r < TT * C; r += 32) {
                     const int tl_l = r / C, c_l = r % C;
@@ -426,9 +500,11 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM, OUT>::THREADS, 1) stft_scm_k
                 }
                 __syncwarp();   // nyq[] is rewritten by the next tile
             }
+            rc.tile();
         }
+        rc.done(RC_ROLE_LOADER);
     } else if (is_fft) {
-        if (G::REALLOC) set_maxnreg<G::REG_FFT, G::REG_LAUNCH>();
+        if (G::REALLOC && !G::DEAL) set_maxnreg<G::REG_FFT, G::REG_LAUNCH>();
         // =========================================================== FFT warps
         // f0 = wf / FFT_WARPS is always 0 and w = wf % FFT_WARPS always wf.  They stay runtime values on purpose: with
         // a constant first tile and a constant barrier id nvcc schedules the FFT loop differently, and the cfg2 / cfg3
@@ -440,13 +516,22 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM, OUT>::THREADS, 1) stft_scm_k
 #pragma unroll
             for (int j = 0; j < RA; ++j) win[j] = p.window[lane + 32 * j];
         }
-        for (int it = f0; it < n_it; ++it) {
+        RoleClocks rc;
+        // the tile an FFT warp is working on: its stages and extent
+        struct FftTile {
+            int s, nfr, c_valid;
+            const float* sm;
+            bool full;
+        };
+        // start tile `it`: wait for its samples, fill the reflect padding of edge tiles (every FFT warp takes part),
+        // wait for its spectrum stage
+        auto enter_tile = [&](int it) {
             int grp, t0;
             tile_of(it, grp, t0);
             const int nfr = min(TT, T - t0), s = it % NSTG, c_valid = min(C, p.n_sig - grp * C);
             const uint32_t ph = (it / NSTG) & 1;
             const float* sm = samp + s * SAMP;
-            mbar_wait(&samp_full[s], ph);
+            rc.wait(RC_SAMP_FULL, &samp_full[s], ph);
             {
                 const int s0 = t0 * H - H;
                 const int cnt = (nfr + 1) * H;
@@ -457,8 +542,9 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM, OUT>::THREADS, 1) stft_scm_k
                     const float* xg = p.x + (size_t)grp * C * L;
                     float* dst = samp + s * SAMP;
                     named_bar_sync(1 + f0, 32 * G::FFT_WARPS);        // every FFT warp is done with this stage
+                    // (DEAL: not unrolled, which helps keep the 104-register FFT warps free of spills; edge tiles only)
                     for (int c = 0; c < c_valid; ++c)
-#pragma unroll 4
+#pragma unroll(G::DEAL ? 1 : 4)
                         for (int q = w * 32 + lane; q < n_fill; q += 32 * G::FFT_WARPS) {
                             const int k = q < k_lo ? q : q + (k_hi - k_lo);
                             int sidx = s0 + k;               // librosa center=True, pad_mode='reflect'
@@ -471,73 +557,105 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM, OUT>::THREADS, 1) stft_scm_k
                     named_bar_sync(1 + f0, 32 * G::FFT_WARPS);
                 }
             }
-            mbar_wait(&spec_empty[s], ph ^ 1);                // spectrum stage s free (tile it-2 consumed)
+            rc.wait(RC_SPEC_EMPTY, &spec_empty[s], ph ^ 1);   // spectrum stage s free (tile it-2 consumed)
             const bool full = (nfr == TT && c_valid == C && (C % 2 == 0) && (G::ITEMS % P == 0));
-#pragma unroll 1
-            for (int jj = 0; jj < G::JPW; ++jj) {
-                const int jb = w * G::JPW + jj;
-                float2* job = spec + s * G::SPEC + (size_t)jb * NB * ROWP;
-                // inter-pass twiddles W_N^(lane k1): fetched once per job, shared by its transforms
-                constexpr bool TWREG = (RA <= 16);
-                float2 twr[TWREG ? RA : 1];
-                if (TWREG) {
+            return FftTile{s, nfr, c_valid, sm, full};
+        };
+        // job jb of tile tc; `release`: the warp's last job of the tile, after which it signals samp_empty
+        auto run_job = [&](const FftTile& tc, int jb, bool release) {
+            const int s = tc.s, nfr = tc.nfr, c_valid = tc.c_valid;
+            const float* sm = tc.sm;
+            const bool full = tc.full;
+            float2* job = spec + s * G::SPEC + (size_t)jb * NB * ROWP;
+            // inter-pass twiddles W_N^(lane k1): fetched once per job, shared by its transforms
+            constexpr bool TWREG = (RA <= 16);
+            float2 twr[TWREG ? RA : 1];
+            if (TWREG) {
 #pragma unroll
-                    for (int k1 = 1; k1 < RA; ++k1) twr[k1] = tw[k1 * 32 + lane];
-                }
+                for (int k1 = 1; k1 < RA; ++k1) twr[k1] = tw[k1 * 32 + lane];
+            }
 #pragma unroll
-                for (int q = 0; q < NB; ++q) {
-                    const int item = jb * NB + q;
-                    const int tl = item / P, pr = item % P;
-                    const int ca = 2 * pr, cb = 2 * pr + 1;
-                    const float* xa = sm + ca * (TT + 1) * H + tl * H + lane;
-                    const float* xb = sm + cb * (TT + 1) * H + tl * H + lane;
-                    float2 v[RA];
-                    if (full || (tl < nfr && cb < c_valid)) {
+            for (int q = 0; q < NB; ++q) {
+                const int item = jb * NB + q;
+                const int tl = item / P, pr = item % P;
+                const int ca = 2 * pr, cb = 2 * pr + 1;
+                const float* xa = sm + ca * (TT + 1) * H + tl * H + lane;
+                const float* xb = sm + cb * (TT + 1) * H + tl * H + lane;
+                float2 v[RA];
+                if (full || (tl < nfr && cb < c_valid)) {
 #pragma unroll
-                        for (int j = 0; j < RA; ++j) {
-                            const float wj = WINREG ? win[j] : p.window[lane + 32 * j];
-                            v[j] = fmul2(make_float2(xa[32 * j], xb[32 * j]), make_float2(wj, wj));
-                        }
-                    } else if (tl < nfr && ca < c_valid) {
-#pragma unroll
-                        for (int j = 0; j < RA; ++j) {
-                            const float wj = WINREG ? win[j] : p.window[lane + 32 * j];
-                            v[j] = make_float2(xa[32 * j] * wj, 0.f);
-                        }
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < RA; ++j) v[j] = make_float2(0.f, 0.f);
+                    for (int j = 0; j < RA; ++j) {
+                        const float wj = WINREG ? win[j] : p.window[lane + 32 * j];
+                        v[j] = fmul2(make_float2(xa[32 * j], xb[32 * j]), make_float2(wj, wj));
                     }
-                    if (jj == G::JPW - 1 && q == NB - 1) {
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive(&samp_empty[s]);   // all samples of this warp are in registers
+                } else if (tl < nfr && ca < c_valid) {
+#pragma unroll
+                    for (int j = 0; j < RA; ++j) {
+                        const float wj = WINREG ? win[j] : p.window[lane + 32 * j];
+                        v[j] = make_float2(xa[32 * j] * wj, 0.f);
                     }
-                    dft_reg<RA, false>(v);
+                } else {
 #pragma unroll
-                    for (int k1 = 1; k1 < RA; ++k1) v[k1] = cmul(v[k1], TWREG ? twr[k1] : tw[k1 * 32 + lane]);
-#pragma unroll
-                    for (int k1 = 0; k1 < RA; ++k1) job[(q * RA + k1) * 33 + lane] = v[k1];   // scratch [32 rows][33]
+                    for (int j = 0; j < RA; ++j) v[j] = make_float2(0.f, 0.f);
                 }
-                __syncwarp();
-                float2 u[32];
-#pragma unroll
-                for (int l = 0; l < 32; ++l) u[l] = job[lane * 33 + l];
-                __syncwarp();
-                dft_reg<32, false>(u);
-                {
-                    float2* row = job + (lane / RA) * ROWP + (lane % RA);
-#pragma unroll
-                    for (int k2 = 0; k2 < 32; ++k2) row[RA * k2] = u[k2];
+                if (release && q == NB - 1) {
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&samp_empty[s]);   // all samples of this warp are in registers
                 }
+                dft_reg<RA, false>(v);
+#pragma unroll
+                for (int k1 = 1; k1 < RA; ++k1) v[k1] = cmul(v[k1], TWREG ? twr[k1] : tw[k1 * 32 + lane]);
+#pragma unroll
+                for (int k1 = 0; k1 < RA; ++k1) job[(q * RA + k1) * 33 + lane] = v[k1];   // scratch [32 rows][33]
             }
             __syncwarp();
-            if (lane == 0) mbar_arrive(&spec_full[s]);
+            float2 u[32];
+#pragma unroll
+            for (int l = 0; l < 32; ++l) u[l] = job[lane * 33 + l];
+            __syncwarp();
+            dft_reg<32, false>(u);
+            {
+                float2* row = job + (lane / RA) * ROWP + (lane % RA);
+#pragma unroll
+                for (int k2 = 0; k2 < 32; ++k2) row[RA * k2] = u[k2];
+            }
+            rc.job();
+        };
+        if constexpr (G::DEAL) {
+            // job j of the CTA's tile stream (tile j / JOBS, job j % JOBS of it) runs on warp j mod FFT_WARPS; with
+            // JOBS >= FFT_WARPS every warp has a job in every tile, so each enters every tile (and its fill) in order.
+            // samp_empty and spec_full count job arrivals.
+            FftTile tc{};
+            int cur = -1;
+#pragma unroll 1
+            for (int j = w; j < n_it * G::JOBS; j += G::FFT_WARPS) {
+                const int it = j / G::JOBS;
+                if (it != cur) {
+                    tc = enter_tile(it);
+                    cur = it;
+                    rc.tile();
+                }
+                run_job(tc, j % G::JOBS, true);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&spec_full[tc.s]);
+            }
+        } else {
+            for (int it = f0; it < n_it; ++it) {
+                const FftTile tc = enter_tile(it);
+#pragma unroll 1
+                for (int jj = 0; jj < G::JPW; ++jj) run_job(tc, w * G::JPW + jj, jj == G::JPW - 1);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&spec_full[tc.s]);
+                rc.tile();
+            }
         }
+        rc.done(RC_ROLE_FFT);
     } else {
         if (G::REALLOC) set_maxnreg<G::REG_SCM, G::REG_LAUNCH>();
         // =========================================================== SCM warps: thread <-> bin f
         const int f = (warp - SCM_WARP0) * 32 + lane;   // 0 .. N/2 - 1
         const int fn = (N - f) & (N - 1);
+        RoleClocks rc;
         if constexpr (FILT) {
             // =========================================================== filter consumer: thread <-> bin f
             float2 w1[C], w2[C];
@@ -567,7 +685,7 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM, OUT>::THREADS, 1) stft_scm_k
                     }
                     dual_filter<C>(w1, w2, y, p.ref, z, zn, yf);
                 };
-                mbar_wait(&spec_full[s], (it / NSTG) & 1);
+                rc.wait(RC_SPEC_FULL, &spec_full[s], (it / NSTG) & 1);
                 if constexpr (!FT) {
                     // frame-major rows, coalesced over the bins of a warp
                     const size_t o = ((size_t)grp * T + t0) * F + f;
@@ -620,7 +738,9 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM, OUT>::THREADS, 1) stft_scm_k
                 }
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&spec_empty[s]);
+                rc.tile();
             }
+            rc.done(RC_ROLE_SCM);
             return;
         }
         ScmAcc<C, NM> acc;
@@ -667,7 +787,7 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM, OUT>::THREADS, 1) stft_scm_k
                     else
                         load_mask(it + 1, 0);
                 }
-                if (ch == 0) mbar_wait(&spec_full[s], (it / NSTG) & 1);
+                if (ch == 0) rc.wait(RC_SPEC_FULL, &spec_full[s], (it / NSTG) & 1);
 #pragma unroll
                 for (int i = 0; i < MC; ++i) {
                     const int tl = ch * MC + i;
@@ -703,7 +823,9 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM, OUT>::THREADS, 1) stft_scm_k
                 acc.flush(p.part + ((size_t)grp * p.slots_per_grp + seg_slot(grp)) * NACC * F + f, F);
                 acc.reset();
             }
+            rc.tile();
         }
+        rc.done(RC_ROLE_SCM);
     }
 }
 
@@ -860,3 +982,25 @@ cudaError_t launch_scm_finalize(const float* part, float2* Rss, float2* Rnn, int
 }
 
 }  // namespace disco
+
+#ifdef DISCO_ROLE_CLOCKS
+// Measurement build only: the layout of the role-clock buffer, [max_ctas][32 warps][slots] unsigned 64-bit values.
+extern "C" __attribute__((visibility("default"))) void disco_role_clocks_layout(int* max_ctas, int* slots) {
+    *max_ctas = disco::RC_MAX_CTAS;
+    *slots = disco::RC_SLOTS;
+}
+// Measurement build only: copy the role clocks of the last stft_scm_kernel launch to host memory `dst` (at most
+// `bytes`) and, with reset != 0, zero them.  Returns the number of bytes copied, or -1 on a CUDA error.
+extern "C" __attribute__((visibility("default"))) long long disco_role_clocks(void* dst, size_t bytes, int reset) {
+    const size_t n = sizeof(disco::g_role_clocks) < bytes ? sizeof(disco::g_role_clocks) : bytes;
+    if (cudaDeviceSynchronize() != cudaSuccess) return -1;
+    if (n && cudaMemcpyFromSymbol(dst, disco::g_role_clocks, n) != cudaSuccess) return -1;
+    if (reset) {
+        void* a = nullptr;
+        if (cudaGetSymbolAddress(&a, disco::g_role_clocks) != cudaSuccess ||
+            cudaMemset(a, 0, sizeof(disco::g_role_clocks)) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess)
+            return -1;
+    }
+    return (long long)n;
+}
+#endif
