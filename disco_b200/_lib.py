@@ -58,6 +58,10 @@ SIGNATURES = {
                                     c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int_p, c_int, c_void_p]),
     "disco_filter_sum_blocks": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
                                         c_int, c_int, c_int, c_int, c_int, c_int_p, c_int, c_void_p]),
+    "disco_stream_stft": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                  c_int, c_int, c_int, c_int, c_void_p]),
+    "disco_stream_istft": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
+                                   c_void_p]),
     "disco_band_stats": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, ctypes.c_longlong, c_int, c_int,
                                  c_void_p]),
     "disco_transpose_c64": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),

@@ -556,6 +556,84 @@ int disco_filter_sum_blocks(const void* W, int conj_w, const void* Y, const void
     return 0;
 }
 
+int disco_stream_stft(const float* hist, const float* chunk, float* hist_out, void* Y, void* Y_blk, int n_sig,
+                      int n_new, int length, int t0, int n_fr, int blk_frames, int blk_slot, int final_call, int n_fft,
+                      void* stream) {
+    if (!valid_nfft(n_fft)) return fail(DISCO_ERR_INVALID, "n_fft must be 256, 512 or 1024");
+    if (n_sig <= 0 || (n_sig + 1) / 2 > kMaxGridYZ) return fail(DISCO_ERR_INVALID, "n_sig must be in 1..131070");
+    if (n_new < 0 || length < n_new || t0 < 0 || n_fr < 0) return fail(DISCO_ERR_INVALID, "bad sizes");
+    if (!hist || (n_new > 0 && !chunk) || (n_fr > 0 && !Y) || (final_call && n_new > 0))
+        return fail(DISCO_ERR_INVALID, "null pointer (or a chunk on the final call)");
+    const int H = n_fft / 2, L0 = length - n_new;
+    if (n_fr > 0) {
+        // every sample the frames read has arrived (the last frame is reflected at the end on the final call), and
+        // the first one lies within the carried history
+        const int t1 = t0 + n_fr - 1;
+        const bool arrived = length > H && (final_call ? t1 <= length / H : (t1 == 0 || (t1 + 1) * H <= length));
+        if (!arrived || (t0 >= 1 && (t0 - 1) * H < L0 - n_fft))
+            return fail(DISCO_ERR_INVALID, "frames not complete, or older than the carried history");
+        if (Y_blk && (blk_slot < 0 || blk_slot + n_fr > blk_frames))
+            return fail(DISCO_ERR_INVALID, "frames outside the block buffer");
+    }
+    Tables tb;
+    int rc = get_tables(n_fft, &tb);
+    if (rc) return rc;
+    StreamStftArgs a;
+    memset(&a, 0, sizeof(a));
+    a.hist = hist;
+    a.chunk = chunk;
+    a.hist_out = hist_out;
+    a.Y = (float2*)Y;
+    a.Y_blk = (float2*)Y_blk;
+    a.twiddle = tb.twiddle;
+    a.window = tb.win_half;
+    a.n_sig = n_sig;
+    a.n_new = n_new;
+    a.length = length;
+    a.t0 = t0;
+    a.n_fr = n_fr;
+    a.blk_frames = blk_frames;
+    a.blk_slot = blk_slot;
+    a.final_call = final_call ? 1 : 0;
+    CU(launch_stream_stft(a, n_fft, (cudaStream_t)stream), "stream_stft launch");
+    return 0;
+}
+
+int disco_stream_istft(const void* Y, float* carry, float* x, int n_sig, int t0, int n_fr, int length, int final_call,
+                       int x_first, int x_stride, int n_fft, void* stream) {
+    if (!valid_nfft(n_fft)) return fail(DISCO_ERR_INVALID, "n_fft must be 256, 512 or 1024");
+    if (n_sig <= 0 || t0 < 0 || n_fr < 0 || length < 1 || x_first < 0 || x_stride < 0)
+        return fail(DISCO_ERR_INVALID, "bad sizes");
+    if (!carry || (n_fr > 0 && !Y)) return fail(DISCO_ERR_INVALID, "null pointer");
+    const int H = n_fft / 2;
+    // samples written: the hop blocks max(t0, 1) .. t0 + n_fr - 1, and on the final call the rest up to length
+    const int lo = (t0 > 0 ? t0 - 1 : 0) * H;
+    int hi = final_call ? length : (t0 + n_fr - 1) * H;
+    if (hi > length) hi = length;
+    if (hi > lo) {
+        if (!x) return fail(DISCO_ERR_INVALID, "null pointer");
+        if (lo < x_first || hi > x_first + x_stride) return fail(DISCO_ERR_INVALID, "output samples outside x");
+    }
+    Tables tb;
+    int rc = get_tables(n_fft, &tb);
+    if (rc) return rc;
+    StreamIstftArgs a;
+    a.Y = (const float2*)Y;
+    a.carry = carry;
+    a.x = x;
+    a.twiddle = tb.twiddle;
+    a.window = tb.win;
+    a.n_sig = n_sig;
+    a.t0 = t0;
+    a.n_fr = n_fr;
+    a.length = length;
+    a.final_call = final_call ? 1 : 0;
+    a.x_first = x_first;
+    a.ld = x_stride;
+    CU(launch_stream_istft(a, n_fft, (cudaStream_t)stream), "stream_istft launch");
+    return 0;
+}
+
 int disco_band_stats(const float* x, const float* sel, const double* ba, double* stats, int n_sig, int length,
                      long long row_stride, int n_band, int order, void* stream) {
     if (!x || !ba || !stats || n_sig < 1 || length < 1 || n_band < 1 || row_stride < length)

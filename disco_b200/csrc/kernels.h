@@ -225,6 +225,30 @@ struct IstftArgs {
 };
 cudaError_t launch_istft(const IstftArgs& a, int n_fft, cudaStream_t st);
 
+// Streaming STFT / iSTFT (stream.cu): disco_stft and disco_istft on a signal that arrives chunk by chunk.
+struct StreamStftArgs {
+    const float* hist;      // [n_sig][N]: samples [L0 - N, L0) of every signal, L0 = length - n_new
+    const float* chunk;     // [n_sig][n_new]: samples [L0, length)
+    float* hist_out;        // [n_sig][N]: samples [length - N, length) written here (null: no update)
+    float2* Y;              // [n_sig][n_fr][F]: frames t0 .. t0 + n_fr - 1
+    float2* Y_blk;          // optional [n_sig][blk_frames][F]: the same frames at slots blk_slot ..
+    const float2* twiddle;  // [N/32][32]
+    const float* window;    // [N]: 0.5 * periodic Hann
+    int n_sig, n_new, length, t0, n_fr, blk_frames, blk_slot;
+    int final_call;         // 1: the stream ends at `length` (reflect padding at the end)
+};
+cudaError_t launch_stream_stft(const StreamStftArgs& a, int n_fft, cudaStream_t st);
+
+struct StreamIstftArgs {
+    const float2* Y;        // [n_sig][n_fr][F]: frames t0 .. t0 + n_fr - 1
+    float* carry;           // [n_sig][N/2]: windowed second half of frame t0 - 1 in, of the last frame out
+    float* x;               // [n_sig][ld]: sample s at x[s - x_first]
+    const float2* twiddle;
+    const float* window;    // [N] periodic Hann (unscaled)
+    int n_sig, t0, n_fr, length, final_call, x_first, ld;
+};
+cudaError_t launch_stream_istft(const StreamIstftArgs& a, int n_fft, cudaStream_t st);
+
 cudaError_t launch_tf_mask(const float2* S, const float2* Nn, float* M, size_t n, int kind, int power,
                            float thr_lin, cudaStream_t st);
 // out[b][c][r] = in[b][r][c]

@@ -476,6 +476,67 @@ def filter_sum_blocks(W, Y, Z=None, block=8, lag=1, conj=True, ref=0, n_fft=512,
 
 
 @_on_device
+def stream_stft(hist, chunk, length, t0, n_fr, n_fft=512, hist_out=None, Y_blk=None, blk_slot=0, final=False):
+    """Frames [t0, t0 + n_fr) of signals that arrive chunk by chunk, equal to those of stft() on the whole signal.
+    hist [..., n_fft] float32 holds samples [L0 - n_fft, L0) of every signal, chunk [..., n] the new samples
+    [L0, length) (n = 0 on the final call, final=True, which reflects the last frame at the end).  hist_out [...,
+    n_fft] (optional) receives samples [length - n_fft, length); Y_blk [..., P, F] (optional) receives the frames at
+    slots blk_slot ...  Returns Y [..., n_fr, F] complex64."""
+    _need(hist, torch.float32, "hist")
+    _need(chunk, torch.float32, "chunk")
+    lead, F = tuple(hist.shape[:-1]), n_fft // 2 + 1
+    if hist.shape[-1] != n_fft or tuple(chunk.shape[:-1]) != lead:
+        raise ValueError("hist %s / chunk %s, expected [..., %d] / [..., n] with the same leading shape"
+                         % (tuple(hist.shape), tuple(chunk.shape), n_fft))
+    n_sig = hist.numel() // n_fft
+    P = 0
+    if hist_out is not None:
+        _need(hist_out, torch.float32, "hist_out")
+        if hist_out.shape != hist.shape or hist_out.data_ptr() == hist.data_ptr():
+            raise ValueError("hist_out must be a second buffer shaped like hist")
+    if Y_blk is not None:
+        _need(Y_blk, torch.complex64, "Y_blk")
+        P = Y_blk.shape[-2]
+        if tuple(Y_blk.shape) != lead + (P, F):
+            raise ValueError("Y_blk shape %s, expected %s" % (tuple(Y_blk.shape), lead + (P, F)))
+    Y = torch.empty(lead + (int(n_fr), F), dtype=torch.complex64, device=hist.device)
+    _lib.check(_lib.load().disco_stream_stft(_ptr(hist), _ptr(chunk) if chunk.numel() else None, _ptr(hist_out),
+                                             _ptr(Y), _ptr(Y_blk), n_sig, chunk.shape[-1], int(length), int(t0),
+                                             int(n_fr), P, int(blk_slot), 1 if final else 0, n_fft, _stream()))
+    return Y
+
+
+@_on_device
+def stream_istft(Y, carry, t0, length, n_fft=512, final=False, x=None, x_first=0):
+    """The hop blocks that frames [t0, t0 + n_fr) of Y [..., n_fr, F] make final, equal to those of istft() on the
+    whole signal: samples [(max(t0, 1) - 1) hop, (t0 + n_fr - 1) hop), and with final=True the rest up to `length`.
+    carry [..., n_fft // 2] float32 (zeros before frame 0) is updated in place.  They are written to x [..., S] at
+    x[..., s - x_first] (x = None: a new tensor starting at the first sample written).  Returns x."""
+    _need(Y, torch.complex64, "Y")
+    _need(carry, torch.float32, "carry")
+    n_fr, F = Y.shape[-2:]
+    H = n_fft // 2
+    lead = tuple(Y.shape[:-2])
+    if F != H + 1 or tuple(carry.shape) != lead + (H,):
+        raise ValueError("Y %s / carry %s, expected [..., n_fr, %d] / [..., %d]" % (tuple(Y.shape), tuple(carry.shape),
+                                                                                    H + 1, H))
+    n_sig = carry.numel() // H
+    lo = max(int(t0) - 1, 0) * H
+    hi = min(int(length), int(length) if final else (int(t0) + n_fr - 1) * H)
+    if x is None:
+        x = torch.empty(lead + (max(hi - lo, 0),), dtype=torch.float32, device=Y.device)
+        x_first = lo
+    else:
+        _need(x, torch.float32, "x")
+        if tuple(x.shape[:-1]) != lead:
+            raise ValueError("x shape %s, expected %s" % (tuple(x.shape), lead + (-1,)))
+    _lib.check(_lib.load().disco_stream_istft(_ptr(Y) if Y.numel() else None, _ptr(carry), _ptr(x) if x.numel() else None,
+                                              n_sig, int(t0), int(n_fr), int(length), 1 if final else 0, int(x_first),
+                                              x.shape[-1], n_fft, _stream()))
+    return x
+
+
+@_on_device
 def band_stats(x, ba, sel=None):
     """IIR filter bank + statistics of every band's output (reference metrics.py:96-110: lfilter, then np.var of
     the selected samples).  x [..., L] float32 (a time slice of a contiguous tensor is taken in place),

@@ -239,6 +239,30 @@ DISCO_API int disco_filter_sum_blocks(const void* W, int conj_w, const void* Y, 
                      int ref, int block, int lag, int n_utt, int K, int C, int T, int n_fft, const int* node_sel,
                      int n_sel, void* stream);
 
+/* ---- streaming STFT / iSTFT (the online Tango session, disco_b200/stream.py) -------------------------
+ * disco_stft and disco_istft of signals that arrive chunk by chunk, equal to the whole-signal calls value for value
+ * (the same pairing of signals 2p, 2p + 1 into one complex transform, the same operations in the same order).
+ * disco_stream_stft computes frames [t0, t0 + n_fr) of n_sig signals whose first `length` samples have arrived:
+ *   hist     [n_sig][n_fft] float32: samples [L0 - n_fft, L0) of every signal, L0 = length - n_new (entries before
+ *            sample 0 are not read)
+ *   chunk    [n_sig][n_new] float32: samples [L0, length) (may be NULL when n_new = 0)
+ *   hist_out [n_sig][n_fft] float32: receives samples [length - n_fft, length), the next call's `hist` (NULL: no
+ *            update; must not alias hist)
+ *   Y        [n_sig][n_fr][F] complex64 out; Y_blk (may be NULL) [n_sig][blk_frames][F] receives the same frames at
+ *            slots blk_slot .. blk_slot + n_fr - 1
+ * Frame t reads samples [t hop - hop, t hop + hop), reflected at the start (librosa center=True); every sample it
+ * reads must have arrived, and frame t0 must start within the history.  final_call = 1 ends the stream at `length`
+ * (n_new = 0): the frames are then reflected at the end too, and frame length / hop is the last one.
+ * disco_stream_istft turns frames [t0, t0 + n_fr) of n_sig spectra Y [n_sig][n_fr][F] into the hop blocks that
+ * become final with them: samples [(max(t0, 1) - 1) hop, (t0 + n_fr - 1) hop), written to x[s - x_first] of rows
+ * x_stride floats apart.  carry [n_sig][n_fft / 2] float32 holds the windowed second half of the previous frame
+ * (zeros before frame 0) and is updated in place.  final_call = 1 also writes the rest of the signal up to `length`. */
+DISCO_API int disco_stream_stft(const float* hist, const float* chunk, float* hist_out, void* Y, void* Y_blk,
+                                int n_sig, int n_new, int length, int t0, int n_fr, int blk_frames, int blk_slot,
+                                int final_call, int n_fft, void* stream);
+DISCO_API int disco_stream_istft(const void* Y, float* carry, float* x, int n_sig, int t0, int n_fr, int length,
+                                 int final_call, int x_first, int x_stride, int n_fft, void* stream);
+
 /* ---- IIR filter bank + band statistics -------------------------------------------------------------
  * Replaces, for every band i of a filter bank, `y = scipy.signal.lfilter(b[i], a[i], x)` followed by the
  * statistics np.var needs, as the reference's frequency-weighted metrics do per third-octave band

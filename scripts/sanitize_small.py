@@ -30,6 +30,16 @@ for (B, K, C, T, n_fft) in ((2, 1, 8, 37, 512), (2, 4, 4, 21, 256), (1, 8, 2, 9,
         o = online.online_mwf(Y, m, Z, block=4, lag=1, n_fft=n_fft)
     torch.cuda.synchronize()
     print("ok wide", B, K, C, T, n_fft, float(Rs.abs().mean()))
+# online Tango stream: streaming STFT / iSTFT with carried history, block buffers, a partial last block
+from disco_b200.stream import OnlineTangoStream
+for (B, K, C, n_fft, block, sizes) in ((3, 1, 3, 256, 4, (100, 0, 700, 1, 2500)), (2, 3, 2, 1024, 2, (513, 3000, 77))):
+    s = OnlineTangoStream(B, K, C, n_fft=n_fft, block=block, lag=1, device=dev)
+    fn = lambda t0, Y, z, zn: (torch.rand(z.shape, device=dev), None)
+    for n in sizes:
+        s.push(torch.randn(B, K, C, n, device=dev), fn)
+    out = s.flush(fn)
+    torch.cuda.synchronize()
+    print("ok stream", B, K, C, n_fft, s.frames_out, s.samples_out, float(out["yf_time"].abs().mean()))
 x = torch.randn(37, 3000, device=dev)
 print("ok bank", float(post.fw_snr(x[:, 100:], 0.5 * torch.randn(37, 2900, device=dev), 16000)[1].mean()))
 torch.cuda.synchronize()
