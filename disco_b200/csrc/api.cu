@@ -489,13 +489,17 @@ int disco_istft(const void* Y, float* x, int n_sig, int T, int length, int n_fft
     int rc = get_tables(n_fft, &tb);
     if (rc) return rc;
     IstftArgs a;
+    memset(&a, 0, sizeof(a));
     a.Y = (const float2*)Y;
     a.x = x;
     a.twiddle = tb.twiddle;
     a.window = tb.win;
     a.n_sig = n_sig;
     a.L = length;
-    a.T = T;
+    a.y_frames = T;
+    a.ld = length;
+    a.j_end = T;
+    a.tail = 1;
     CU(launch_istft(a, n_fft, (cudaStream_t)stream), "istft launch");
     return 0;
 }
@@ -617,20 +621,23 @@ int disco_stream_istft(const void* Y, float* carry, float* x, int n_sig, int t0,
     Tables tb;
     int rc = get_tables(n_fft, &tb);
     if (rc) return rc;
-    StreamIstftArgs a;
+    IstftArgs a;
+    memset(&a, 0, sizeof(a));
     a.Y = (const float2*)Y;
-    a.carry = carry;
     a.x = x;
+    a.carry = carry;
     a.twiddle = tb.twiddle;
     a.window = tb.win;
     a.n_sig = n_sig;
-    a.t0 = t0;
-    a.n_fr = n_fr;
-    a.length = length;
-    a.final_call = final_call ? 1 : 0;
-    a.x_first = x_first;
+    a.L = length;
+    a.y_frames = n_fr;
+    a.y_t0 = t0;
     a.ld = x_stride;
-    CU(launch_stream_istft(a, n_fft, (cudaStream_t)stream), "stream_istft launch");
+    a.x_first = x_first;
+    a.j_begin = t0;
+    a.j_end = t0 + n_fr;
+    a.tail = final_call ? 1 : 0;
+    CU(launch_istft(a, n_fft, (cudaStream_t)stream), "stream_istft launch");
     return 0;
 }
 

@@ -1,17 +1,20 @@
-// Inverse STFT with overlap-add and window-sum-square normalisation, batched.
+// Inverse STFT with overlap-add and window-sum-square normalisation, batched: disco_istft over whole signals and
+// disco_stream_istft over the new frames of a stream run one kernel body (istft_body), so a stream's time samples
+// equal those of the whole-signal call value for value.
 //
 // Replaces lb.core.istft(S, hop_length=N/2, win_length=N, center=True, length=L)
 // (reference tango.py:528-539, math_utils.py:143-152; librosa <= 0.9 semantics, SURVEY App. A.2):
 //   per frame irfft -> * periodic Hann -> overlap-add -> divide by overlap-added window^2 where
 //   it exceeds tiny(float32) -> drop N/2 leading samples -> crop / zero-pad to L.
 //
-// One CTA owns a PAIR of signals and a chunk of frames.  The two real inverse transforms are done
+// One CTA owns a PAIR of signals and a chunk of hop blocks.  The two real inverse transforms are done
 // by one complex inverse FFT: Z[k] = A[k] + i B[k] (k <= N/2), Z[N-k] = conj(A[k]) + i conj(B[k]),
 // so Re z = a, Im z = b.  The FFT itself is the same two-pass in-register scheme as the forward
 // kernel (stft_scm.cu) with conjugated twiddles.  With 50 % overlap every output hop block j
 // (samples [(j-1) hop, j hop)) is  w[n] frame_j[n] + w[n+hop] frame_{j-1}[n+hop]; the second half of
-// the last frame of a tile is carried in shared memory to the next tile, and a chunk recomputes
-// the one frame before its first block, so there are no atomics and the result is deterministic.
+// the last frame of a tile is carried in shared memory to the next tile.  Over a whole signal a chunk
+// recomputes the one frame before its first block, so there are no atomics and the result is deterministic;
+// a stream carries that half frame between calls in a global buffer instead.
 #include "common.cuh"
 #include "fft_reg.cuh"
 #include "kernels.h"
@@ -25,10 +28,14 @@ struct IGeom {
     static constexpr int FFT_WARPS = N / 64;
     static constexpr int THREADS = N / 2 + 32;
     static constexpr int ITEMS = 16;
+    static constexpr size_t SMEM = (size_t)ITEMS * ROW * sizeof(float2) + H * sizeof(float2) + N * sizeof(float2) +
+                                   N * sizeof(float);
 };
 
-template <int N>
-__global__ void __launch_bounds__(IGeom<N>::THREADS) istft_kernel(IstftArgs p, int frames_per_chunk, int T_eff) {
+// The body of both kernels below.  STREAM is a template parameter, not a test of p.carry, so that the whole-signal
+// kernel keeps its own machine code: with the stream's carry and offsets as runtime cases it ran 4 % slower.
+template <int N, bool STREAM>
+DISCO_DEV void istft_body(const IstftArgs& p) {
     using G = IGeom<N>;
     constexpr int RA = G::RA, NB = G::NB, H = G::H, F = G::F, ROW = G::ROW, TT = G::ITEMS;
     extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -41,22 +48,26 @@ __global__ void __launch_bounds__(IGeom<N>::THREADS) istft_kernel(IstftArgs p, i
     const int pair = blockIdx.y, chunk = blockIdx.x;
     const int sa = 2 * pair, sb = 2 * pair + 1;
     const bool has_b = sb < p.n_sig;
-    const int T = p.T, L = p.L;
-    const float2* Ya = p.Y + (size_t)sa * T * F;
-    const float2* Yb = p.Y + (size_t)(has_b ? sb : sa) * T * F;
-    float* xa = p.x + (size_t)sa * L;
-    float* xb = p.x + (size_t)(has_b ? sb : sa) * L;
+    const int L = p.L;
+    const int y_t0 = STREAM ? p.y_t0 : 0, x_first = STREAM ? p.x_first : 0;
+    // (the stream's b rows are offsets from the a rows: as pointers of their own they spill at 1024 points)
+    const float2* Ya = p.Y + (size_t)sa * p.y_frames * F;                 // frame j at row j - y_t0
+    const float2* Yb = STREAM ? Ya + (has_b ? (size_t)p.y_frames * F : 0) : p.Y + (size_t)(has_b ? sb : sa) * p.y_frames * F;
+    float* xa = p.x + (size_t)sa * p.ld;                                  // sample s at s - x_first
+    float* xb = STREAM ? xa + (has_b ? (size_t)p.ld : 0) : p.x + (size_t)(has_b ? sb : sa) * p.ld;
 
-    const int j_begin = chunk * frames_per_chunk;                 // first hop block of this chunk
-    const int j_end = min(T_eff, j_begin + frames_per_chunk);     // blocks [j_begin, j_end) (+ T_eff if last)
-    const bool last_chunk = (j_end == T_eff);
-    const int fs = max(j_begin - 1, 0);                           // first frame to transform
+    const int j_begin = (STREAM ? p.j_begin : 0) + chunk * p.fpc;   // first hop block of this chunk
+    const int j_end = min(p.j_end, j_begin + p.fpc);              // blocks [j_begin, j_end) (+ j_end with the tail)
+    const bool tail = (!STREAM || p.tail) && j_end == p.j_end;
+    const int fs = STREAM ? j_begin : max(j_begin - 1, 0);       // first frame to transform
 
     for (int i = tid; i < N; i += blockDim.x) {
         tw[i] = p.twiddle[i];
         win[i] = p.window[i];
     }
-    if (tid < H) carry[tid] = make_float2(0.f, 0.f);
+    if (tid < H)
+        carry[tid] = STREAM ? make_float2(p.carry[(size_t)sa * H + tid], has_b ? p.carry[(size_t)sb * H + tid] : 0.f)
+                             : make_float2(0.f, 0.f);
     __syncthreads();
     const float inv_n = 1.0f / (float)N;
     const float tiny = 1.17549435e-38f;
@@ -67,7 +78,7 @@ __global__ void __launch_bounds__(IGeom<N>::THREADS) istft_kernel(IstftArgs p, i
         if (tid < F) {
             const int f = tid;
             for (int tl = 0; tl < nfr; ++tl) {
-                const size_t off = (size_t)(t0 + tl) * F + f;
+                const size_t off = (size_t)(t0 + tl - y_t0) * F + f;
                 float2 A = Ya[off];
                 float2 B = has_b ? Yb[off] : make_float2(0.f, 0.f);
                 float2* row = rows + tl * ROW;
@@ -126,8 +137,8 @@ __global__ void __launch_bounds__(IGeom<N>::THREADS) istft_kernel(IstftArgs p, i
                     if (wss > tiny) val = cscale(val, 1.0f / wss);
                     const int s = (j - 1) * H + n;
                     if (s >= 0 && s < L) {
-                        xa[s] = val.x;
-                        if (has_b) xb[s] = val.y;
+                        xa[s - x_first] = val.x;
+                        if (has_b) xb[s - x_first] = val.y;
                     }
                 }
                 prev = cscale(nxt, w1 * inv_n);
@@ -136,50 +147,66 @@ __global__ void __launch_bounds__(IGeom<N>::THREADS) istft_kernel(IstftArgs p, i
         }
         __syncthreads();
     }
-    // ---- tail: block T_eff has only the second half of the last frame; then zero-fill up to L
-    if (last_chunk) {
+    if (STREAM && tid < H) {
+        p.carry[(size_t)sa * H + tid] = carry[tid].x;
+        if (has_b) p.carry[(size_t)sb * H + tid] = carry[tid].y;
+    }
+    // ---- tail: block j_end has only the second half of the last frame; then zero-fill up to L
+    if (tail) {
         if (tid < H) {
             const int n = tid;
             const float w1 = win[n + H];
             float2 val = carry[n];
             const float wss = w1 * w1;
             if (wss > tiny) val = cscale(val, 1.0f / wss);
-            const int s = (T_eff - 1) * H + n;
+            const int s = (j_end - 1) * H + n;
             if (s >= 0 && s < L) {
-                xa[s] = val.x;
-                if (has_b) xb[s] = val.y;
+                xa[s - x_first] = val.x;
+                if (has_b) xb[s - x_first] = val.y;
             }
         }
-        for (int s = T_eff * H + tid; s < L; s += blockDim.x) {
-            xa[s] = 0.f;
-            if (has_b) xb[s] = 0.f;
+        for (int s = j_end * H + tid; s < L; s += blockDim.x) {
+            xa[s - x_first] = 0.f;
+            if (has_b) xb[s - x_first] = 0.f;
         }
     }
 }
 
 template <int N>
-static cudaError_t launch_n(const IstftArgs& a, cudaStream_t st) {
+__global__ void __launch_bounds__(IGeom<N>::THREADS) istft_kernel(IstftArgs p) {
+    istft_body<N, false>(p);
+}
+template <int N>
+__global__ void __launch_bounds__(IGeom<N>::THREADS) stream_istft_kernel(IstftArgs p) {
+    istft_body<N, true>(p);
+}
+
+template <int N>
+static cudaError_t launch_n(IstftArgs a, cudaStream_t st) {
     using G = IGeom<N>;
     const int H = G::H;
-    int T_eff = min(a.T, (a.L + N + H - 1) / H);
-    if (T_eff < 1) return cudaErrorInvalidValue;
     const int pairs = (a.n_sig + 1) / 2;
     int chunks = 1;
-    while (pairs * chunks < sm_count() * 2 && (T_eff + chunks - 1) / chunks > 4 * G::ITEMS) chunks *= 2;
-    int fpc = ((T_eff + chunks - 1) / chunks + G::ITEMS - 1) / G::ITEMS * G::ITEMS;
-    chunks = (T_eff + fpc - 1) / fpc;
-    const size_t smem = (size_t)G::ITEMS * G::ROW * sizeof(float2) + H * sizeof(float2) + N * sizeof(float2) +
-                        N * sizeof(float);
-    auto kern = istft_kernel<N>;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (!a.carry) {   // whole signals: the blocks past the last sample are not computed; chunks of fpc blocks
+        a.j_end = min(a.j_end, (a.L + N + H - 1) / H);
+        const int T_eff = a.j_end - a.j_begin;
+        if (T_eff < 1) return cudaErrorInvalidValue;
+        while (pairs * chunks < sm_count() * 2 && (T_eff + chunks - 1) / chunks > 4 * G::ITEMS) chunks *= 2;
+        a.fpc = ((T_eff + chunks - 1) / chunks + G::ITEMS - 1) / G::ITEMS * G::ITEMS;
+        chunks = (T_eff + a.fpc - 1) / a.fpc;
+    } else {          // a stream: one CTA per pair runs all the new blocks
+        a.fpc = a.j_end - a.j_begin;
+    }
+    auto kern = a.carry ? stream_istft_kernel<N> : istft_kernel<N>;
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G::SMEM);
     if (e != cudaSuccess) return e;
     dim3 grid(chunks, pairs);
-    kern<<<grid, G::THREADS, smem, st>>>(a, fpc, T_eff);
+    kern<<<grid, G::THREADS, G::SMEM, st>>>(a);
     return cudaGetLastError();
 }
 
 cudaError_t launch_istft(const IstftArgs& a, int n_fft, cudaStream_t st) {
-    if (a.n_sig <= 0) return cudaSuccess;
+    if (a.n_sig <= 0 || (a.j_end <= a.j_begin && !a.tail)) return cudaSuccess;
     switch (n_fft) {
         case 256: return launch_n<256>(a, st);
         case 512: return launch_n<512>(a, st);

@@ -216,16 +216,25 @@ struct BankArgs {
 };
 cudaError_t launch_band_stats(const BankArgs& a, int order, cudaStream_t st);
 
+// Hop blocks [j_begin, j_end) of the iSTFT of every signal (istft.cu).  Whole signals (carry == null): blocks
+// [0, T), the launcher drops those past L and splits the rest into chunks of fpc blocks, each of which recomputes
+// the frame before its first block.  A stream (disco_stream_istft): the blocks of frames t0 .. t0 + n_fr - 1, one
+// CTA per signal pair, the windowed half frame before them carried in `carry`.
 struct IstftArgs {
-    const float2* Y;     // [n_sig][T][F] frame-major complex64
-    float* x;            // [n_sig][L]
+    const float2* Y;        // frame j of signal s at Y + (s * y_frames + j - y_t0) * F, frame-major complex64
+    float* x;               // sample i of signal s at x[s * ld + i - x_first]
+    float* carry;           // null, or [n_sig][N/2]: windowed second half of frame j_begin - 1 in, of frame j_end - 1 out
     const float2* twiddle;
-    const float* window; // [N] periodic Hann (unscaled)
-    int n_sig, L, T;
+    const float* window;    // [N] periodic Hann (unscaled)
+    int n_sig, L;           // signals, samples per signal
+    int y_frames, y_t0, ld, x_first;
+    int j_begin, j_end;
+    int fpc;                // blocks per chunk (grid.x); set by the launcher
+    int tail;               // 1: also block j_end (second half of frame j_end - 1) and the zero fill up to L
 };
 cudaError_t launch_istft(const IstftArgs& a, int n_fft, cudaStream_t st);
 
-// Streaming STFT / iSTFT (stream.cu): disco_stft and disco_istft on a signal that arrives chunk by chunk.
+// Streaming STFT (stream.cu): disco_stft on a signal that arrives chunk by chunk.
 struct StreamStftArgs {
     const float* hist;      // [n_sig][N]: samples [L0 - N, L0) of every signal, L0 = length - n_new
     const float* chunk;     // [n_sig][n_new]: samples [L0, length)
@@ -238,16 +247,6 @@ struct StreamStftArgs {
     int final_call;         // 1: the stream ends at `length` (reflect padding at the end)
 };
 cudaError_t launch_stream_stft(const StreamStftArgs& a, int n_fft, cudaStream_t st);
-
-struct StreamIstftArgs {
-    const float2* Y;        // [n_sig][n_fr][F]: frames t0 .. t0 + n_fr - 1
-    float* carry;           // [n_sig][N/2]: windowed second half of frame t0 - 1 in, of the last frame out
-    float* x;               // [n_sig][ld]: sample s at x[s - x_first]
-    const float2* twiddle;
-    const float* window;    // [N] periodic Hann (unscaled)
-    int n_sig, t0, n_fr, length, final_call, x_first, ld;
-};
-cudaError_t launch_stream_istft(const StreamIstftArgs& a, int n_fft, cudaStream_t st);
 
 cudaError_t launch_tf_mask(const float2* S, const float2* Nn, float* M, size_t n, int kind, int power,
                            float thr_lin, cudaStream_t st);

@@ -20,7 +20,7 @@
 //   FFT warps     two real channels are transformed by ONE complex FFT.  A job is 32/RA transforms
 //                          (RA = N/32): an RA-point in-register DFT per lane, a padded transposition
 //                          through shared memory, then one 32-point in-register DFT per lane
-//                          (fft_reg.cuh).  Spectra of the pairs stay in smem.
+//                          (stft_core.cuh, shared with stream.cu).  Spectra of the pairs stay in smem.
 //   SCM warps     thread f owns frequency bin f.  It un-mixes the two-for-one spectra, writes Y
 //                          (frame-major rows, coalesced), and accumulates the Hermitian upper
 //                          triangles of  sum_t m^2 y y^H  and  sum_t (1-m)^2 y y^H  (per mask) in
@@ -37,8 +37,8 @@
 // segment into a small workspace and reduced in fixed order by scm_finalize_kernel or directly by
 // the solver (deterministic, no atomics).
 #include "common.cuh"
-#include "fft_reg.cuh"
 #include "kernels.h"
+#include "stft_core.cuh"
 
 namespace disco {
 
@@ -49,15 +49,11 @@ namespace disco {
 enum : int { OUT_Y = 0, OUT_NONE = 1, OUT_FILTER = 2, OUT_FILTER_FT = 3 };
 
 template <int N, int C, int NM = 1, int OUT = OUT_Y>
-struct StftCfg {
-    static constexpr int RA = N / 32;              // radix of the per-lane first pass
-    static constexpr int NB = 32 / RA;             // transforms per warp job
-    static constexpr int HALF = N / 2;             // hop (50 % overlap)
-    static constexpr int F = N / 2 + 1;            // bins
+struct StftCfg : StftJob<N> {                      // RA, NB, H, F, ROWP: the FFT job (stft_core.cuh)
     static constexpr bool WIDE = C > 4;            // 128 accumulators per bin
     static constexpr int NSTG = 2;                 // pipeline stages (samples and spectra)
     static constexpr int JOBS = 8;                 // jobs per tile
-    static constexpr int ITEMS = JOBS * NB;        // (frame, channel-pair) transforms per tile
+    static constexpr int ITEMS = JOBS * StftJob<N>::NB;   // (frame, channel-pair) transforms per tile
     static constexpr int P = (C + 1) / 2;          // channel pairs per frame
     static constexpr int TT = ITEMS / P;           // frames per tile
     // Roles on warpgroup boundaries + setmaxnreg: the SCM warps of wide arrays (128 accumulators) and of
@@ -76,13 +72,12 @@ struct StftCfg {
     static constexpr int FFT_WARPS = DEAL ? 7 : (N == 512 && (WIDE || NM == 2)) ? 4 : 8;
     static constexpr int JPW = JOBS / FFT_WARPS;   // jobs per FFT warp and tile (without DEAL)
     static constexpr int FFT_ARRIVALS = DEAL ? JOBS : FFT_WARPS;   // samp_empty / spec_full arrivals per tile
-    static constexpr int ROWP = 1056 / NB;         // spectrum row pitch (complex): a job = 32 x 33 scratch
     static constexpr int SCM_WARPS = N / 64;       // bins 0 .. N/2-1, one per thread
     static constexpr int LEAD_WARPS = (REALLOC && !DEAL) ? 4 : 1;   // warp 0 = loader; 1..3 idle (warpgroup padding)
     static constexpr int WARPS = LEAD_WARPS + FFT_WARPS + SCM_WARPS;
     static constexpr int THREADS = 32 * WARPS;
-    static constexpr int SPEC = ITEMS * ROWP;      // complex per spectrum stage
-    static constexpr int SAMP = C * (TT + 1) * HALF;   // floats per sample stage
+    static constexpr int SPEC = ITEMS * StftJob<N>::ROWP;   // complex per spectrum stage
+    static constexpr int SAMP = C * (TT + 1) * StftJob<N>::H;   // floats per sample stage
     // registers per thread at launch: each of the 4 SM sub-partitions holds 16384 registers and ceil(WARPS/4) warps
     static constexpr int REG_LAUNCH = 16384 / ((WARPS + 3) / 4) / 32 / 8 * 8;
     // REALLOC only: setmaxnreg budgets per thread of the roles.  The sm_90a build of every 256- and 512-point
@@ -274,7 +269,7 @@ struct StftParam<OUT_FILTER_FT> {
 template <int N, int C, int NM, int OUT>
 __global__ void __launch_bounds__(StftCfg<N, C, NM, OUT>::THREADS, 1) stft_scm_kernel(typename StftParam<OUT>::type p) {
     using G = StftCfg<N, C, NM, OUT>;
-    constexpr int RA = G::RA, NB = G::NB, H = G::HALF, F = G::F, ROWP = G::ROWP, P = G::P, TT = G::TT;
+    constexpr int RA = G::RA, NB = G::NB, H = G::H, F = G::F, ROWP = G::ROWP, P = G::P, TT = G::TT;
     constexpr int SAMP = G::SAMP;
     constexpr int NACC = NM * 2 * C * C;
     constexpr int NMX = NM > 0 ? NM : 1;
@@ -426,7 +421,7 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM, OUT>::THREADS, 1) stft_scm_k
 #pragma unroll
                     for (int c = 0; c < C; ++c) {
                         const float2 z = spec[s * G::SPEC + (size_t)(lane * P + c / 2) * ROWP + N / 2];
-                        y[c] = make_float2((c & 1) ? z.y + z.y : z.x + z.x, 0.f);
+                        y[c] = make_float2(stft_nyquist(z, c & 1), 0.f);
                     }
                     float2 z, zn, yf;
                     dual_filter<C>(nw1, nw2, y, p.ref, z, zn, yf);
@@ -448,6 +443,7 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM, OUT>::THREADS, 1) stft_scm_k
                     float yv = 0.f;
                     if (tl_l < nfr && c_l < c_valid) {
                         const float2 z = spec[s * G::SPEC + (size_t)(tl_l * P + c_l / 2) * ROWP + N / 2];
+                        // stft_nyquist(z, c_l & 1), written out: the helper changes this path's machine code
                         yv = (c_l & 1) ? z.y + z.y : z.x + z.x;
                         if (STORE_Y) p.Y[(((size_t)grp * C + c_l) * T + t0 + tl_l) * F + (F - 1)] = make_float2(yv, 0.f);
                     }
@@ -547,9 +543,7 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM, OUT>::THREADS, 1) stft_scm_k
 #pragma unroll(G::DEAL ? 1 : 4)
                         for (int q = w * 32 + lane; q < n_fill; q += 32 * G::FFT_WARPS) {
                             const int k = q < k_lo ? q : q + (k_hi - k_lo);
-                            int sidx = s0 + k;               // librosa center=True, pad_mode='reflect'
-                            if (sidx < 0) sidx = -sidx;
-                            if (sidx >= L) sidx = 2 * (L - 1) - sidx;
+                            const int sidx = reflect_index(s0 + k, L);
                             float v = 0.f;
                             if (sidx >= 0 && sidx < L) v = xg[(size_t)c * L + sidx];
                             dst[c * (TT + 1) * H + k] = v;
@@ -602,23 +596,9 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM, OUT>::THREADS, 1) stft_scm_k
                     __syncwarp();
                     if (lane == 0) mbar_arrive(&samp_empty[s]);   // all samples of this warp are in registers
                 }
-                dft_reg<RA, false>(v);
-#pragma unroll
-                for (int k1 = 1; k1 < RA; ++k1) v[k1] = cmul(v[k1], TWREG ? twr[k1] : tw[k1 * 32 + lane]);
-#pragma unroll
-                for (int k1 = 0; k1 < RA; ++k1) job[(q * RA + k1) * 33 + lane] = v[k1];   // scratch [32 rows][33]
+                stft_pass1<RA, TWREG>(v, job, q, lane, twr, tw);
             }
-            __syncwarp();
-            float2 u[32];
-#pragma unroll
-            for (int l = 0; l < 32; ++l) u[l] = job[lane * 33 + l];
-            __syncwarp();
-            dft_reg<32, false>(u);
-            {
-                float2* row = job + (lane / RA) * ROWP + (lane % RA);
-#pragma unroll
-                for (int k2 = 0; k2 < 32; ++k2) row[RA * k2] = u[k2];
-            }
+            stft_pass2<RA>(job, lane);
             rc.job();
         };
         if constexpr (G::DEAL) {
@@ -679,9 +659,10 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM, OUT>::THREADS, 1) stft_scm_k
 #pragma unroll
                     for (int pr = 0; pr < P; ++pr) {
                         const float2* row = stage + (size_t)(tl * P + pr) * ROWP;
-                        const float2 zf = row[f], zb = row[fn];
-                        y[2 * pr] = fadd2(zf, make_float2(zb.x, -zb.y));
-                        if (2 * pr + 1 < C) y[2 * pr + 1] = fadd2(make_float2(zf.y, -zf.x), make_float2(zb.y, zb.x));
+                        float2 ya, yb;
+                        stft_unmix(row[f], row[fn], ya, yb);
+                        y[2 * pr] = ya;
+                        if (2 * pr + 1 < C) y[2 * pr + 1] = yb;
                     }
                     dual_filter<C>(w1, w2, y, p.ref, z, zn, yf);
                 };
@@ -792,15 +773,15 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM, OUT>::THREADS, 1) stft_scm_k
                 for (int i = 0; i < MC; ++i) {
                     const int tl = ch * MC + i;
                     if (tl < TT && (full || tl < nfr)) {
-                        // un-mix the two-for-one spectra (window carries the 1/2):
-                        //   A = Z[f] + conj(Z[N-f]),  B = -i (Z[f] - conj(Z[N-f]))
+                        // un-mix the two-for-one spectra
                         float2 y[C];
 #pragma unroll
                         for (int pr = 0; pr < P; ++pr) {
                             const float2* row = stage + (size_t)(tl * P + pr) * ROWP;
-                            const float2 zf = row[f], zn = row[fn];
-                            y[2 * pr] = fadd2(zf, make_float2(zn.x, -zn.y));
-                            if (2 * pr + 1 < C) y[2 * pr + 1] = fadd2(make_float2(zf.y, -zf.x), make_float2(zn.y, zn.x));
+                            float2 ya, yb;
+                            stft_unmix(row[f], row[fn], ya, yb);
+                            y[2 * pr] = ya;
+                            if (2 * pr + 1 < C) y[2 * pr + 1] = yb;
                         }
                         if (STORE_Y) {
 #pragma unroll
