@@ -64,7 +64,10 @@ SIGNATURES = {
                                    c_void_p]),
     "disco_band_stats": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, ctypes.c_longlong, c_int, c_int,
                                  c_void_p]),
-    "disco_transpose_c64": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "disco_bss_eval_workspace": (c_size_t, [c_int, c_int, c_int, c_int, c_int]),
+    "disco_bss_eval": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_size_t,
+                               c_void_p]),
+    "disco_transpose_c64":(c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "disco_transpose_f32": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "disco_apply_mask": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_int, c_void_p]),
     "disco_apply_mask_channels": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_int, c_size_t, c_int, c_void_p]),

@@ -660,6 +660,43 @@ int disco_band_stats(const float* x, const float* sel, const double* ba, double*
     return 0;
 }
 
+static int bss_check(int n_set, int nsrc, int n_est, int length, int flen) {
+    if (n_set < 1 || n_est < 1 || length < 1 || nsrc < 1) return fail(DISCO_ERR_INVALID, "bad sizes");
+    if (flen < 1 || flen > kBssMaxFlen) return fail(DISCO_ERR_INVALID, "flen must be in 1..512");
+    if (nsrc > kBssMaxSrc) return fail(DISCO_ERR_UNSUPPORTED, "bss_eval: at most 4 reference sources");
+    if ((long long)n_set * nsrc > 0x7fffffffLL || (nsrc + n_est + 3) / 4 > kMaxGridYZ ||
+        (length + kBssSeg - 1) / kBssSeg > kMaxGridYZ)
+        return fail(DISCO_ERR_UNSUPPORTED, "bss_eval: too many sets, estimates or samples for one call");
+    return 0;
+}
+
+size_t disco_bss_eval_workspace(int n_set, int nsrc, int n_est, int length, int flen) {
+    if (bss_check(n_set, nsrc, n_est, length, flen)) return 0;
+    return bss_ws_doubles(n_set, nsrc, n_est, length, flen) * sizeof(double);
+}
+
+int disco_bss_eval(const float* refs, const float* ests, double* norms, int n_set, int nsrc, int n_est, int length,
+                   int flen, void* workspace, size_t workspace_bytes, void* stream) {
+    int rc = bss_check(n_set, nsrc, n_est, length, flen);
+    if (rc) return rc;
+    if (!refs || !ests || !norms) return fail(DISCO_ERR_INVALID, "null pointer");
+    if (!workspace || workspace_bytes < bss_ws_doubles(n_set, nsrc, n_est, length, flen) * sizeof(double))
+        return fail(DISCO_ERR_WORKSPACE, "workspace too small");
+    BssArgs a;
+    memset(&a, 0, sizeof(a));
+    a.refs = refs;
+    a.ests = ests;
+    a.norms = norms;
+    a.part = (double*)workspace;
+    a.n_set = n_set;
+    a.nsrc = nsrc;
+    a.n_est = n_est;
+    a.L = length;
+    a.flen = flen;
+    CU(launch_bss_eval(a, (cudaStream_t)stream), "bss_eval launch");
+    return 0;
+}
+
 int disco_transpose_c64(const void* in, void* out, int batch, int rows, int cols, void* stream) {
     if (!in || !out) return fail(DISCO_ERR_INVALID, "null pointer");
     if (batch > kMaxGridYZ) return fail(DISCO_ERR_UNSUPPORTED, "at most 65535 planes per call");

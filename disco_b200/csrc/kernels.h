@@ -216,6 +216,24 @@ struct BankArgs {
 };
 cudaError_t launch_band_stats(const BankArgs& a, int order, cudaStream_t st);
 
+// BSS-eval squared norms (bss.cu; mir_eval.separation.bss_eval_sources as tango.main calls it).
+constexpr int kBssMaxSrc = 4;         // references per set
+constexpr int kBssMaxFlen = 512;      // mir_eval's filter length
+constexpr int kBssSeg = 4096;         // samples per correlation time segment
+constexpr double kBssDelta = 1e-10;   // a pivot <= kBssDelta * max diag G marks a dependent column
+struct BssArgs {
+    const float* refs;   // [n_set][nsrc][L]
+    const float* ests;   // [n_set][n_est][L]
+    double* norms;       // [n_set][n_est][1 + 2 nsrc]: ‖e‖², ‖y_all‖² per reference block, ‖y_k‖² of each reference alone
+    double* part;        // workspace: segment partial correlations, then the rest (set by the launcher)
+    double* corr;
+    double* mat;
+    size_t mat_per_set;
+    int n_set, nsrc, n_est, L, flen, n_seg;
+};
+size_t bss_ws_doubles(int n_set, int nsrc, int n_est, int L, int flen);
+cudaError_t launch_bss_eval(BssArgs a, cudaStream_t st);
+
 // Hop blocks [j_begin, j_end) of the iSTFT of every signal (istft.cu).  Whole signals (carry == null): blocks
 // [0, T), the launcher drops those past L and splits the rest into chunks of fpc blocks, each of which recomputes
 // the frame before its first block.  A stream (disco_stream_istft): the blocks of frames t0 .. t0 + n_fr - 1, one

@@ -570,6 +570,43 @@ def band_stats(x, ba, sel=None):
     return stats
 
 
+# Device scratch of one disco_bss_eval call (the Gram matrices and their factors, ~11 MB per reference set of 2
+# sources at flen 512); larger batches of sets run in consecutive chunks.
+BSS_WORKSPACE_CAP = 1 << 30
+
+
+@_on_device
+def bss_eval(refs, ests, flen=512):
+    """Float64 projection norms of BSS-eval (disco_bss_eval).  refs [S, nsrc, L], ests [S, R, L] float32 (R estimate
+    rows per reference set) -> norms [S, R, 1 + 2 nsrc] float64: ‖e‖², the part of ‖P_all e‖² from each reference's
+    block, ‖P_k e‖² of each reference alone.  Sets are processed in chunks whose workspace stays within
+    BSS_WORKSPACE_CAP bytes (one set at least)."""
+    _need(refs, torch.float32, "refs")
+    _need(ests, torch.float32, "ests")
+    if refs.dim() != 3 or ests.dim() != 3 or ests.shape[0] != refs.shape[0] or ests.shape[2] != refs.shape[2]:
+        raise ValueError("refs [S, nsrc, L] / ests [S, R, L] shape mismatch: %s / %s"
+                         % (tuple(refs.shape), tuple(ests.shape)))
+    S, nsrc, L = refs.shape
+    R = ests.shape[1]
+    if nsrc > 4:
+        raise NotImplementedError("bss_eval: at most 4 reference sources (got %d)" % nsrc)
+    lib = _lib.load()
+    norms = torch.empty((S, R, 1 + 2 * nsrc), dtype=torch.float64, device=refs.device)
+    if S == 0:
+        return norms
+    per_set = lib.disco_bss_eval_workspace(1, nsrc, R, L, int(flen))
+    if per_set == 0:
+        _lib.check(lib.disco_bss_eval(None, None, None, 1, nsrc, R, L, int(flen), None, 0, _stream()))
+    chunk = max(1, min(S, BSS_WORKSPACE_CAP // per_set))
+    ws_bytes = lib.disco_bss_eval_workspace(chunk, nsrc, R, L, int(flen))
+    ws = torch.empty(ws_bytes // 8, dtype=torch.float64, device=refs.device)
+    for s0 in range(0, S, chunk):
+        n = min(chunk, S - s0)
+        _lib.check(lib.disco_bss_eval(_ptr(refs[s0:s0 + n]), _ptr(ests[s0:s0 + n]), _ptr(norms[s0:s0 + n]), n, nsrc,
+                                      R, L, int(flen), _ptr(ws), ws_bytes, _stream()))
+    return norms
+
+
 @_on_device
 def transpose_last2(a):
     """[..., R, C] -> [..., C, R] (contiguous) for complex64 / float32 device tensors."""

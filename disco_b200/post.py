@@ -6,7 +6,9 @@ the device.  Mirrors the post-processing of disco_theque/speech_enhancement/tang
 (metrics.py:63-128, 211-279) run the whole third-octave Butterworth bank over all signals in one launch of
 the IIR filter-bank kernel (csrc/filterbank.cu) that returns only the band powers; the band weighting is a
 few float64 operations on [..., 17] tensors.  `si_sdr`, `snr`, `sd` are float64 reductions (torch on the
-device).  The third-party `bss_eval` / STOI scores of tango.main stay outside this repository's scope.
+device).  BSS-eval's SDR / SIR / SAR (mir_eval.separation.bss_eval_sources) run on the float64 projection kernels of
+csrc/bss.cu (disco_b200/bss_eval.py); `tango_scores` is the whole scoring block of tango.main without STOI, whose
+third-party implementation stays outside this repository's scope.
 
 All metrics are batched: TIME IS THE LAST AXIS, every leading axis is a batch axis (the reference's
 functions take one 1-D signal per call).
@@ -177,3 +179,51 @@ def sd(s_out, s_in, db=True):
     """metrics.py:48-62."""
     r = _var_nonzero(s_in) / _var_nonzero(s_out)
     return 10.0 * torch.log10(r) if db else r
+
+
+def tango_scores(y, s, n, s_dry, n_dry, times, fs):
+    """The scoring block of the reference's tango.main (tango.py:541-593) without STOI, batched over utterances and
+    nodes.  y, s, n [B, K, L]: mixture, target and noise at each node's reference microphone; s_dry, n_dry [B, L_dry]
+    the dry sources of every utterance; times: the to_time() outputs ('yf', 'z_y', 'sf', 'nf', 'z_s', 'z_n', each
+    [B, K, L]); float32 CUDA tensors.  Every signal is cut to [fs:min_len] as the reference does.
+    Returns (results, resultsz) [B, K] float64 tensors keyed like the reference's two result pickles, without
+    'delta_stoi*' and without 'snr_in_raw' (the caller's SNRs).
+
+    bss(refs, ests) is only read at row 0, and row 0's scores depend on no other estimate row, so only the first row
+    of each estimate set is correlated: (sh, szh, y) against the node's (s, n), and the same rows of all K nodes of an
+    utterance against its dry (s_dry, n_dry), whose Gram matrix is factored once for the K nodes."""
+    from . import bss_eval
+    B, K, L = y.shape
+    min_len = min(L, times["yf"].shape[-1], s_dry.shape[-1], n_dry.shape[-1])
+    cut = lambda x: x[..., fs:min_len]
+    sh, szh, yy = cut(times["yf"]), cut(times["z_y"]), cut(y)
+    sf, nf, szf, nzf = cut(times["sf"]), cut(times["nf"]), cut(times["z_s"]), cut(times["z_n"])
+    ss, nn, sd_, nd_ = cut(s), cut(n), cut(s_dry), cut(n_dry)
+    rows = torch.stack((sh, szh, yy), dim=2)                                     # [B, K, 3, Ls]
+    refs = torch.stack((ss, nn), dim=2)                                          # [B, K, 2, Ls]
+    sdr, sir, sar = bss_eval.first_row_scores(refs.contiguous(), rows.contiguous())          # [B, K, 3]
+    refs_dry = torch.stack((sd_, nd_), dim=1)                                    # [B, 2, Ls]
+    d_sdr, d_sir, d_sar = bss_eval.first_row_scores(refs_dry.contiguous(),
+                                                    rows.reshape(B, K * 3, -1).contiguous())
+    d_sdr, d_sir, d_sar = (x.view(B, K, 3) for x in (d_sdr, d_sir, d_sar))
+
+    _, snr_out, _ = fw_snr(sf, nf, fs)
+    _, snr_in, _ = fw_snr(ss, nn, fs)
+    _, snr_in_dry, _ = fw_snr(sd_, nd_, fs)
+    _, snr_out_z, _ = fw_snr(szf, nzf, fs)
+    snr_in_dry = snr_in_dry.unsqueeze(1).expand(B, K)
+    _, sd_cnv, _ = fw_sd(sf, ss, fs)
+    _, sd_dry, _ = fw_sd(sf, sd_.unsqueeze(1).expand(B, K, -1), fs)
+    _, sd_cnv_z, _ = fw_sd(szf, ss, fs)
+    _, sd_dry_z, _ = fw_sd(szf, sd_.unsqueeze(1).expand(B, K, -1), fs)
+
+    shared = {"snr_in_cnv": snr_in, "snr_in_dry": snr_in_dry,
+              "sdr_in_cnv": sdr[..., 2], "sir_in_cnv": sir[..., 2],
+              "sdr_in_dry": d_sdr[..., 2], "sir_in_dry": d_sir[..., 2], "sar_in_dry": d_sar[..., 2]}
+    results = {"sar_cnv": sar[..., 0], "sir_cnv": sir[..., 0], "sdr_cnv": sdr[..., 0],
+               "snr_out": snr_out, "fw_sd_cnv": sd_cnv, "fw_sd_dry": sd_dry,
+               "sar_dry": d_sar[..., 0], "sir_dry": d_sir[..., 0], "sdr_dry": d_sdr[..., 0], **shared}
+    resultsz = {"sar_cnv": sar[..., 1], "sir_cnv": sir[..., 1], "sdr_cnv": sdr[..., 1],
+                "snr_out": snr_out_z, "fw_sd_cnv": sd_cnv_z, "fw_sd_dry": sd_dry_z,
+                "sar_dry": d_sar[..., 1], "sir_dry": d_sir[..., 1], "sdr_dry": d_sdr[..., 1], **shared}
+    return results, resultsz

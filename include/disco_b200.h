@@ -275,6 +275,24 @@ DISCO_API int disco_stream_istft(const void* Y, float* carry, float* x, int n_si
 DISCO_API int disco_band_stats(const float* x, const float* sel, const double* ba, double* stats, int n_sig, int length,
                      long long row_stride, int n_band, int order, void* stream);
 
+/* ---- BSS-eval source scores (float64) -----------------------------------------------------------------
+ * Replaces the projections of mir_eval.separation.bss_eval_sources (called six times per node by the reference's
+ * evaluation, tango.py:552-567) for n_set reference sets at once.  For set s with references r_1 .. r_nsrc and every
+ * estimate row e of it, A_S holds the references of S delayed by 0 .. flen-1 samples (zero-padded), P_S e is the
+ * least-squares projection of e onto A_S, and ‖P_S e‖² = ‖y_S‖², L_S y_S = A_S^T e, L_S L_S^T = A_S^T A_S.
+ *   refs  [n_set][nsrc][length] float32, ests [n_set][n_est][length] float32
+ *   norms [n_set][n_est][1 + 2 nsrc] float64 out:
+ *         [0]             ‖e‖²
+ *         [1 + b]         the part of ‖y_all‖² (all references) from reference b's block, b < nsrc (sum = ‖P_all e‖²)
+ *         [1 + nsrc + k]  ‖y_k‖² = ‖P_k e‖² of reference k alone
+ * nsrc 1..4 (more: DISCO_ERR_UNSUPPORTED), flen 1..512 (mir_eval uses 512), length >= 1.  A Cholesky pivot below
+ * 1e-10 times the largest diagonal entry of the Gram matrix marks its column as linearly dependent: the projection is
+ * then onto the span of the remaining columns (what a least-squares solve gives for a singular Gram matrix).
+ * workspace: disco_bss_eval_workspace() bytes (0 for invalid sizes); it grows with n_set: batch in chunks. */
+DISCO_API size_t disco_bss_eval_workspace(int n_set, int nsrc, int n_est, int length, int flen);
+DISCO_API int disco_bss_eval(const float* refs, const float* ests, double* norms, int n_set, int nsrc, int n_est,
+                             int length, int flen, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- layout helpers -------------------------------------------------------------------------------
  * out[b][c][r] = in[b][r][c] for `batch` planes (complex64 / float32).  Used at the Python
  * boundary to move between the reference (F, T) layout and the native (T, F) layout. */
