@@ -606,8 +606,8 @@ int disco_stream_stft(const float* hist, const float* chunk, float* hist_out, vo
 int disco_stream_istft(const void* Y, float* carry, float* x, int n_sig, int t0, int n_fr, int length, int final_call,
                        int x_first, int x_stride, int n_fft, void* stream) {
     if (!valid_nfft(n_fft)) return fail(DISCO_ERR_INVALID, "n_fft must be 256, 512 or 1024");
-    if (n_sig <= 0 || t0 < 0 || n_fr < 0 || length < 1 || x_first < 0 || x_stride < 0)
-        return fail(DISCO_ERR_INVALID, "bad sizes");
+    if (n_sig <= 0 || (n_sig + 1) / 2 > kMaxGridYZ) return fail(DISCO_ERR_INVALID, "n_sig must be in 1..131070");
+    if (t0 < 0 || n_fr < 0 || length < 1 || x_first < 0 || x_stride < 0) return fail(DISCO_ERR_INVALID, "bad sizes");
     if (!carry || (n_fr > 0 && !Y)) return fail(DISCO_ERR_INVALID, "null pointer");
     const int H = n_fft / 2;
     // samples written: the hop blocks max(t0, 1) .. t0 + n_fr - 1, and on the final call the rest up to length

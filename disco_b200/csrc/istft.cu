@@ -200,9 +200,24 @@ static cudaError_t launch_n(IstftArgs a, cudaStream_t st) {
     auto kern = a.carry ? stream_istft_kernel<N> : istft_kernel<N>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G::SMEM);
     if (e != cudaSuccess) return e;
-    dim3 grid(chunks, pairs);
-    kern<<<grid, G::THREADS, G::SMEM, st>>>(a);
-    return cudaGetLastError();
+    if (a.carry) {    // the stream's signal count is bounded by its ABI (one launch of at most kMaxGridYZ pairs)
+        kern<<<dim3(chunks, pairs), G::THREADS, G::SMEM, st>>>(a);
+        return cudaGetLastError();
+    }
+    // pairs sit in grid.y: whole signals run in consecutive launches of at most kMaxGridYZ pairs, each starting at an
+    // even signal (a pair keeps its partner) with Y and x advanced to it (whole-signal rows are contiguous per signal)
+    const int n_sig = a.n_sig, F = N / 2 + 1;
+    for (int p0 = 0; p0 < pairs; p0 += kMaxGridYZ) {
+        IstftArgs b = a;
+        const int s0 = 2 * p0;
+        b.Y = a.Y + (size_t)s0 * a.y_frames * F;
+        b.x = a.x + (size_t)s0 * a.ld;
+        b.n_sig = min(n_sig - s0, 2 * kMaxGridYZ);
+        kern<<<dim3(chunks, (b.n_sig + 1) / 2), G::THREADS, G::SMEM, st>>>(b);
+        e = cudaGetLastError();
+        if (e != cudaSuccess) return e;
+    }
+    return cudaSuccess;
 }
 
 cudaError_t launch_istft(const IstftArgs& a, int n_fft, cudaStream_t st) {

@@ -40,26 +40,33 @@ cudaError_t launch_tf_mask(const float2* S, const float2* Nn, float* M, size_t n
     return cudaGetLastError();
 }
 
+// 32 x 32 tiles: column tiles in grid.x, planes in grid.z; grid.y strides over the row tiles, so a plane of any
+// number of rows (T frames of a long recording) fits the 65535 limit of grid.y
 template <typename T>
 __global__ void transpose_kernel(const T* __restrict__ in, T* __restrict__ out, int rows, int cols) {
     __shared__ T tile[32][33];
     const size_t base = (size_t)blockIdx.z * rows * cols;
-    const int c0 = blockIdx.x * 32, r0 = blockIdx.y * 32;
-    for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-        const int r = r0 + i, c = c0 + threadIdx.x;
-        if (r < rows && c < cols) tile[i][threadIdx.x] = in[base + (size_t)r * cols + c];
-    }
-    __syncthreads();
-    for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-        const int c = c0 + i, r = r0 + threadIdx.x;
-        if (r < rows && c < cols) out[base + (size_t)c * rows + r] = tile[threadIdx.x][i];
+    const int c0 = blockIdx.x * 32, row_tiles = (rows + 31) / 32;
+    for (int rt = blockIdx.y; rt < row_tiles; rt += gridDim.y) {
+        const int r0 = rt * 32;
+        for (int i = threadIdx.y; i < 32; i += blockDim.y) {
+            const int r = r0 + i, c = c0 + threadIdx.x;
+            if (r < rows && c < cols) tile[i][threadIdx.x] = in[base + (size_t)r * cols + c];
+        }
+        __syncthreads();
+        for (int i = threadIdx.y; i < 32; i += blockDim.y) {
+            const int c = c0 + i, r = r0 + threadIdx.x;
+            if (r < rows && c < cols) out[base + (size_t)c * rows + r] = tile[threadIdx.x][i];
+        }
+        __syncthreads();   // the tile is refilled by the next row tile
     }
 }
 
 template <typename T>
 static cudaError_t launch_transpose(const T* in, T* out, int batch, int rows, int cols, cudaStream_t st) {
     if (batch <= 0 || rows <= 0 || cols <= 0) return cudaSuccess;
-    dim3 grid((cols + 31) / 32, (rows + 31) / 32, batch), block(32, 8);
+    const int row_tiles = (rows + 31) / 32;
+    dim3 grid((cols + 31) / 32, row_tiles < kMaxGridYZ ? row_tiles : kMaxGridYZ, batch), block(32, 8);
     transpose_kernel<T><<<grid, block, 0, st>>>(in, out, rows, cols);
     return cudaGetLastError();
 }

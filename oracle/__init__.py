@@ -20,6 +20,8 @@ ref_shim     Imports the UNMODIFIED reference from /root/reference (only where i
              is mounted) through sys.modules stubs for its absent third-party
              imports; used by make_golden.py to pin the restatement.
 make_golden  Generates tests/golden/*.npz by running the real reference.
+lfilter_np   scipy.signal.lfilter's direct form II transposed restated one ufunc
+             per operation, bit-equal to scipy; the yardstick of band_stats.
 
 Parity pinning status: the reference ships no golden vectors for this path
 (SURVEY.md §4).  The MWF mathematics (SCM, intern_filter, filter-and-sum, the

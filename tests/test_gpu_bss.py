@@ -77,6 +77,21 @@ CASES = [   # nsrc, E, L, flen, kind
     (4, 1, 1, 16, "white"),          # one sample: every G singular beyond rank 16
     (4, 3, 5000, 512, "white"),
     (4, 1, 300, 512, "lowpass"),     # singular
+    # appended estimate rows (E nsrc) spanning 2 and 3 64-row blocks of the factor kernel
+    (2, 33, 1000, 64, "white"),
+    (2, 66, 700, 64, "white"),
+    # nsrc flen around multiples of 64 (the factor's column blocks), flen 1, and M = nsrc (1 + E) at every
+    # remainder mod 4 (the last 4-signal CTA of the correlation kernel)
+    (1, 1, 500, 1, "white"),
+    (4, 1, 2000, 7, "lowpass"),      # 28
+    (4, 2, 3000, 9, "white"),        # 36
+    (1, 2, 3000, 63, "white"),       # 63, M = 3
+    (1, 4, 3000, 65, "lowpass"),     # 65, M = 5
+    (2, 1, 3000, 63, "white"),       # 126
+    (2, 2, 3000, 65, "lowpass"),     # 130
+    (2, 1, 8191, 511, "white"),      # 1022; L one below two 4096-sample segments
+    (3, 2, 8192, 65, "lowpass"),     # 195, M = 9; exactly two segments
+    (3, 4, 12289, 63, "white"),      # 189, M = 15; one sample into a fourth segment
 ]
 
 
@@ -152,7 +167,7 @@ def test_poisoned_outputs_and_workspace(dev):
     G = 512
     lib = _lib.load()
     rng = np.random.default_rng(2)
-    for nsrc, R, L, flen in ((2, 3, 5000, 512), (3, 2, 300, 64), (1, 5, 4096, 100)):
+    for nsrc, R, L, flen in ((2, 3, 5000, 512), (3, 2, 300, 64), (1, 5, 4096, 100), (2, 66, 1000, 64)):
         refs = torch.from_numpy(np.stack([refs_of(rng, nsrc, L, "white") for _ in range(2)])).to(dev)
         ests = torch.from_numpy(rng.standard_normal((2, R, L)).astype(np.float32)).to(dev)
         n = 2 * R * (1 + 2 * nsrc)
@@ -168,6 +183,63 @@ def test_poisoned_outputs_and_workspace(dev):
         assert not bool(torch.isnan(out).any())
         want = ops.bss_eval(refs, ests, flen=flen).reshape(-1)
         assert torch.equal(out, want)
+
+
+def exact_normal_equations(refs, ests, flen):
+    """G = AᵀA and D = Aᵀe of the delayed references, assembled from correctly rounded correlations
+    Q[i][s][k] = Σ_t x_s(t) r_i(t - k) (math.fsum of float64 products of float32 inputs, each exact)."""
+    import math
+    r, e = refs.astype(np.float64), ests.astype(np.float64)
+    nsrc, L = r.shape
+    n = nsrc * flen
+    corr = lambda x, y, k: math.fsum(x[k:] * y[:L - k]) if k < L else 0.0
+    Q = {(i, j, k): corr(r[j], r[i], k) for i in range(nsrc) for j in range(nsrc) for k in range(flen)}
+    G = np.empty((n, n))
+    for i in range(nsrc):
+        for j in range(nsrc):
+            for a in range(flen):
+                for b in range(flen):
+                    G[i * flen + a, j * flen + b] = Q[i, j, a - b] if a >= b else Q[j, i, b - a]
+    D = np.array([[corr(e[q], r[j], b) for q in range(len(e))] for j in range(nsrc) for b in range(flen)])
+    ee = np.array([math.fsum(x * x) for x in e])
+    return G, D, ee
+
+
+@pytest.mark.parametrize("nsrc,R,flen,L", [(1, 3, 64, 700), (2, 4, 64, 1400), (3, 2, 32, 1000), (4, 2, 16, 700)])
+def test_norms_against_float64_cholesky(dev, nsrc, R, flen, L):
+    """The raw norms of ops.bss_eval, entry-wise, against float64 Cholesky of the exactly assembled G and D, for
+    white references (L >= 10 nsrc flen, so G is well conditioned).
+
+    ‖e‖²: a sum of L positive terms, |Δ| <= L 2⁻⁵³ ‖e‖².  Block norms ‖y_b‖², y = L_G⁻¹ D: the device's correlations
+    perturb G and D by at most L 2⁻⁵³ |A|ᵀ|A| and L 2⁻⁵³ |A|ᵀ|e| (n = nsrc flen columns, ‖|A|‖ <= √n ‖A‖), and the
+    Cholesky with its appended rows is backward stable with (n + 1) 2⁻⁵³ n ‖G‖, so with η = (L + n + 1) n 2⁻⁵³ each
+    side errs by at most (η κ(G) + 2 η √(n κ(G))) ‖e‖² <= 3 η κ(G) ‖e‖² (‖y‖ <= ‖e‖); device and host together:
+    |Δ‖y_b‖²| <= 6 η κ(G) ‖e‖².  The dB comparison above cannot see this: its 1e-6 dB floor is ~2e-7 relative."""
+    import scipy.linalg
+    from disco_b200 import ops
+    rng = np.random.default_rng(nsrc * 1000 + R)
+    n = nsrc * flen
+    assert L >= 10 * n
+    refs = refs_of(rng, nsrc, L, "white")
+    ests = np.concatenate([ests_of(rng, refs, 1, (10.0,))[0], rng.standard_normal((R - nsrc, L)).astype(np.float32)]
+                          if R > nsrc else [ests_of(rng, refs, 1, (10.0,))[0][:R]])
+    got = ops.bss_eval(torch.from_numpy(refs[None]).to(dev), torch.from_numpy(ests[None]).to(dev), flen=flen)
+    got = got[0].cpu().numpy()                                           # [R, 1 + 2 nsrc]
+    G, D, ee = exact_normal_equations(refs, ests, flen)
+    kappa = np.linalg.cond(G)
+    eta = (L + n + 1) * n * 2.0 ** -53
+    tol = 6 * eta * kappa * ee
+    np.testing.assert_array_less(np.abs(got[:, 0] - ee), L * 2.0 ** -53 * ee + 1e-300)
+    y = scipy.linalg.solve_triangular(np.linalg.cholesky(G), D, lower=True)            # [n, R]
+    for b in range(nsrc):
+        blk = (y[b * flen:(b + 1) * flen] ** 2).sum(0)
+        assert np.all(np.abs(got[:, 1 + b] - blk) <= tol), (b, got[:, 1 + b], blk, tol)
+        sl = slice(b * flen, (b + 1) * flen)
+        ys = scipy.linalg.solve_triangular(np.linalg.cholesky(G[sl, sl]), D[sl], lower=True)
+        single = (ys ** 2).sum(0)
+        assert np.all(np.abs(got[:, 1 + nsrc + b] - single) <= tol), (b, got[:, 1 + nsrc + b], single, tol)
+    # negative control: an error of 100 times the bound in one block norm is caught
+    assert not np.all(np.abs(got[:, 1] + 100 * tol - (y[:flen] ** 2).sum(0)) <= tol)
 
 
 def test_tango_scores_against_numpy_loop(dev):
