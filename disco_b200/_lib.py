@@ -67,6 +67,10 @@ SIGNATURES = {
     "disco_bss_eval_workspace": (c_size_t, [c_int, c_int, c_int, c_int, c_int]),
     "disco_bss_eval": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_size_t,
                                c_void_p]),
+    "disco_resample_poly": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "disco_stoi_workspace": (c_size_t, [c_int, c_int, c_int]),
+    "disco_stoi": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                           c_void_p, c_size_t, c_void_p]),
     "disco_transpose_c64":(c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "disco_transpose_f32": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "disco_apply_mask": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_int, c_void_p]),

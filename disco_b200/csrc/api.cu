@@ -697,6 +697,69 @@ int disco_bss_eval(const float* refs, const float* ests, double* norms, int n_se
     return 0;
 }
 
+static long long gcd_ll(long long a, long long b) { return b == 0 ? a : gcd_ll(b, a % b); }
+
+int disco_resample_poly(const float* x, double* y, const double* taps, int n_taps, int up, int down, int n_sig,
+                        int length, void* stream) {
+    if (n_taps < 1 || up < 1 || down < 1 || n_sig < 1 || length < 1) return fail(DISCO_ERR_INVALID, "bad sizes");
+    if (gcd_ll(up, down) != 1 || (up == 1 && down == 1))
+        return fail(DISCO_ERR_INVALID, "up and down must be coprime and not both 1");
+    const long long n_out = ((long long)length * up + down - 1) / down;
+    if (n_out > 0x7fffffffLL || (long long)n_sig * ((n_out + 255) / 256) > 0x7fffffffLL)
+        return fail(DISCO_ERR_INVALID, "resample_poly: too many output samples for one call");
+    if (!x || !y || !taps) return fail(DISCO_ERR_INVALID, "null pointer");
+    ResampleArgs a;
+    a.x = x;
+    a.y = y;
+    a.taps = taps;
+    a.n_taps = n_taps;
+    a.up = up;
+    a.down = down;
+    a.n_sig = n_sig;
+    a.n_in = length;
+    a.n_out = (int)n_out;
+    CU(launch_resample_poly(a, (cudaStream_t)stream), "resample_poly launch");
+    return 0;
+}
+
+static int stoi_check(int n_clean, int n_deg, int n_pair, int length) {
+    if (n_clean < 1 || n_deg < 1 || n_pair < 1) return fail(DISCO_ERR_INVALID, "bad sizes");
+    if (length < kStoiFrame) return fail(DISCO_ERR_INVALID, "stoi: signals need at least 256 samples");
+    const long long groups = (stoi_n_fr(length) - 1 + 3) / 4;
+    if (((long long)n_clean + n_pair) * groups > 0x7fffffffLL)
+        return fail(DISCO_ERR_INVALID, "stoi: too many signals or samples for one call");
+    return 0;
+}
+
+size_t disco_stoi_workspace(int n_clean, int n_pair, int length) {
+    if (stoi_check(n_clean, 1, n_pair, length)) return 0;
+    return stoi_ws_bytes(n_clean, n_pair, length);
+}
+
+int disco_stoi(const double* cleans, const double* degraded, const int* pairs, double* d, int* n_sel, int* n_frames,
+               int n_clean, int n_deg, int n_pair, int length, void* workspace, size_t workspace_bytes, void* stream) {
+    int rc = stoi_check(n_clean, n_deg, n_pair, length);
+    if (rc) return rc;
+    if (!cleans || !degraded || !pairs || !d || !n_sel || !n_frames) return fail(DISCO_ERR_INVALID, "null pointer");
+    if (!workspace || workspace_bytes < stoi_ws_bytes(n_clean, n_pair, length))
+        return fail(DISCO_ERR_WORKSPACE, "workspace too small");
+    StoiArgs a;
+    memset(&a, 0, sizeof(a));
+    a.cleans = cleans;
+    a.degraded = degraded;
+    a.pairs = pairs;
+    a.d = d;
+    a.n_sel = n_sel;
+    a.n_frames = n_frames;
+    a.energy = (double*)workspace;
+    a.n_clean = n_clean;
+    a.n_deg = n_deg;
+    a.n_pair = n_pair;
+    a.L = length;
+    CU(launch_stoi(a, (cudaStream_t)stream), "stoi launch");
+    return 0;
+}
+
 int disco_transpose_c64(const void* in, void* out, int batch, int rows, int cols, void* stream) {
     if (!in || !out) return fail(DISCO_ERR_INVALID, "null pointer");
     if (batch > kMaxGridYZ) return fail(DISCO_ERR_UNSUPPORTED, "at most 65535 planes per call");

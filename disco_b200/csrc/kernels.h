@@ -234,6 +234,35 @@ struct BssArgs {
 size_t bss_ws_doubles(int n_set, int nsrc, int n_est, int L, int flen);
 cudaError_t launch_bss_eval(BssArgs a, cudaStream_t st);
 
+// Polyphase resampler with scipy.signal.resample_poly's alignment and gain (stoi.cu).
+struct ResampleArgs {
+    const float* x;      // [n_sig][n_in]
+    double* y;           // [n_sig][n_out], n_out = ceil(n_in up / down)
+    const double* taps;  // [n_taps] scipy's `window` (the gain `up` is applied in the kernel, as scipy does)
+    int n_taps, up, down, n_sig, n_in, n_out;
+};
+cudaError_t launch_resample_poly(const ResampleArgs& a, cudaStream_t st);
+
+// Classic STOI (pystoi 0.3) of 10 kHz float64 signals (stoi.cu).
+constexpr int kStoiFrame = 256;   // frame length; frames start every kStoiFrame / 2 samples
+constexpr int kStoiBands = 15;    // one-third octave bands
+constexpr int kStoiSeg = 30;      // STFT frames per segment
+struct StoiArgs {
+    const double* cleans;    // [n_clean][L]
+    const double* degraded;  // [n_deg][L]
+    const int* pairs;        // [n_pair][2]: clean index, degraded index
+    double* d;               // [n_pair]
+    int* n_sel;              // [n_clean]: frames kept by the silent-frame removal
+    int* n_frames;           // [n_pair]: STFT frames scored (n_sel of the pair's clean - 1; -1 for a bad pair)
+    double* energy;          // workspace [n_clean][n_fr]
+    int* sel;                // workspace [n_clean][n_fr]: kept frame indices, in order
+    double* tob;             // workspace [n_clean + n_pair][n_fr][kStoiBands]: band envelopes
+    int n_clean, n_deg, n_pair, L, n_fr;
+};
+int stoi_n_fr(int L);
+size_t stoi_ws_bytes(int n_clean, int n_pair, int L);
+cudaError_t launch_stoi(StoiArgs a, cudaStream_t st);
+
 // Hop blocks [j_begin, j_end) of the iSTFT of every signal (istft.cu).  Whole signals (carry == null): blocks
 // [0, T), the launcher drops those past L and splits the rest into chunks of fpc blocks, each of which recomputes
 // the frame before its first block.  A stream (disco_stream_istft): the blocks of frames t0 .. t0 + n_fr - 1, one

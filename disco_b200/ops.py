@@ -6,6 +6,7 @@ Layouts: spectra are frame-major ``[..., T, F]`` complex64; ``layout='FT'`` argu
 reference's NumPy layout ``[..., F, T]`` for masks / final outputs (SURVEY.md §8b op table).
 """
 import ctypes
+import math
 
 import torch
 
@@ -605,6 +606,90 @@ def bss_eval(refs, ests, flen=512):
         _lib.check(lib.disco_bss_eval(_ptr(refs[s0:s0 + n]), _ptr(ests[s0:s0 + n]), _ptr(norms[s0:s0 + n]), n, nsrc,
                                       R, L, int(flen), _ptr(ws), ws_bytes, _stream()))
     return norms
+
+
+@_on_device
+def resample_poly(x, taps, up, down):
+    """scipy.signal.resample_poly(x, up, down, window=taps) along the last axis (disco_resample_poly).
+    x [..., L] float32, taps [n] float64 (scipy's `window`; the gain `up` is applied inside) -> [..., ceil(L up / down)]
+    float64.  up and down are reduced by their gcd first, as scipy does; equal rates return x as float64."""
+    _need(x, torch.float32, "x")
+    _need(taps, torch.float64, "taps")
+    up, down = int(up), int(down)
+    if up < 1 or down < 1:
+        raise ValueError("up and down must be >= 1")
+    g = math.gcd(up, down)
+    up, down = up // g, down // g
+    if up == down == 1:
+        return x.double()
+    L = x.shape[-1]
+    n_out = -(-L * up // down)
+    y = torch.empty(x.shape[:-1] + (n_out,), dtype=torch.float64, device=x.device)
+    n_sig = x.numel() // L if L else 0
+    if n_sig == 0:
+        return y
+    _lib.check(_lib.load().disco_resample_poly(_ptr(x), _ptr(y), _ptr(taps), taps.numel(), up, down, n_sig, L,
+                                               _stream()))
+    return y
+
+
+# Device scratch of one disco_stoi call (energies and kept-frame lists of every clean, band envelopes of every clean
+# and every pair: ~85 KB per spectrogram of 9 s); larger batches of pairs run in consecutive chunks.
+STOI_WORKSPACE_CAP = 1 << 30
+
+
+@_on_device
+def stoi(cleans, degraded, pairs):
+    """Classic STOI of 10 kHz signals (disco_stoi).  cleans [C, L], degraded [D, L] float64, pairs [P, 2] int32
+    (clean index, degraded index) -> d [P] float64 (1e-5 below 30 STFT frames), n_sel [C] int32 (frames kept by the
+    silent-frame removal; -1 for a clean no pair names), n_frames [P] int32 (STFT frames scored).  Pairs are processed
+    in chunks whose workspace stays within STOI_WORKSPACE_CAP bytes (one pair at least); a chunk computes only the
+    cleans its pairs name, each once."""
+    _need(cleans, torch.float64, "cleans")
+    _need(degraded, torch.float64, "degraded")
+    _need(pairs, torch.int32, "pairs")
+    if cleans.dim() != 2 or degraded.dim() != 2 or pairs.dim() != 2 or pairs.shape[1] != 2 or \
+            degraded.shape[1] != cleans.shape[1]:
+        raise ValueError("cleans [C, L] / degraded [D, L] / pairs [P, 2] shape mismatch: %s / %s / %s"
+                         % (tuple(cleans.shape), tuple(degraded.shape), tuple(pairs.shape)))
+    C, L = cleans.shape
+    D, P = degraded.shape[0], pairs.shape[0]
+    if L < 256:
+        raise ValueError("stoi: signals of %d samples at 10 kHz; at least 256 are needed" % L)
+    dev = cleans.device
+    d = torch.empty(P, dtype=torch.float64, device=dev)
+    n_frames = torch.empty(P, dtype=torch.int32, device=dev)
+    n_sel = torch.full((C,), -1, dtype=torch.int32, device=dev)
+    if P == 0:
+        return d, n_sel, n_frames
+    if C == 0 or D == 0 or int(pairs[:, 0].min()) < 0 or int(pairs[:, 0].max()) >= C or \
+            int(pairs[:, 1].min()) < 0 or int(pairs[:, 1].max()) >= D:
+        raise IndexError("stoi: pair indices out of range (%d cleans, %d degraded signals)" % (C, D))
+    lib = _lib.load()
+    per_pair = lib.disco_stoi_workspace(1, 1, L)
+    if per_pair == 0:
+        _lib.check(lib.disco_stoi(None, None, None, None, None, None, 1, 1, 1, L, None, 0, _stream()))
+    if lib.disco_stoi_workspace(C, P, L) <= STOI_WORKSPACE_CAP:
+        ws_bytes = lib.disco_stoi_workspace(C, P, L)
+        ws = torch.empty(ws_bytes // 8 + 1, dtype=torch.float64, device=dev)
+        _lib.check(lib.disco_stoi(_ptr(cleans), _ptr(degraded), _ptr(pairs), _ptr(d), _ptr(n_sel), _ptr(n_frames), C,
+                                  D, P, L, _ptr(ws), ws_bytes, _stream()))
+        named = torch.zeros(C, dtype=torch.bool, device=dev)
+        named[pairs[:, 0].long()] = True
+        return d, n_sel.masked_fill_(~named, -1), n_frames
+    chunk = max(1, STOI_WORKSPACE_CAP // per_pair)
+    ws_bytes = lib.disco_stoi_workspace(min(chunk, C), chunk, L)
+    ws = torch.empty(ws_bytes // 8 + 1, dtype=torch.float64, device=dev)
+    for p0 in range(0, P, chunk):
+        n = min(chunk, P - p0)
+        used, local = torch.unique(pairs[p0:p0 + n, 0], return_inverse=True)
+        sub = cleans.index_select(0, used)
+        pr = torch.stack((local.to(torch.int32), pairs[p0:p0 + n, 1]), dim=1).contiguous()
+        sel = torch.empty(used.numel(), dtype=torch.int32, device=dev)
+        _lib.check(lib.disco_stoi(_ptr(sub), _ptr(degraded), _ptr(pr), _ptr(d[p0:]), _ptr(sel), _ptr(n_frames[p0:]),
+                                  used.numel(), D, n, L, _ptr(ws), ws_bytes, _stream()))
+        n_sel[used] = sel
+    return d, n_sel, n_frames
 
 
 @_on_device

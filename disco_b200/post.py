@@ -7,8 +7,8 @@ the device.  Mirrors the post-processing of disco_theque/speech_enhancement/tang
 the IIR filter-bank kernel (csrc/filterbank.cu) that returns only the band powers; the band weighting is a
 few float64 operations on [..., 17] tensors.  `si_sdr`, `snr`, `sd` are float64 reductions (torch on the
 device).  BSS-eval's SDR / SIR / SAR (mir_eval.separation.bss_eval_sources) run on the float64 projection kernels of
-csrc/bss.cu (disco_b200/bss_eval.py); `tango_scores` is the whole scoring block of tango.main without STOI, whose
-third-party implementation stays outside this repository's scope.
+csrc/bss.cu (disco_b200/bss_eval.py) and STOI (pystoi.stoi.stoi) on the float64 kernels of csrc/stoi.cu
+(disco_b200/stoi.py); `tango_scores` is the whole scoring block of tango.main, STOI included on request.
 
 All metrics are batched: TIME IS THE LAST AXIS, every leading axis is a batch axis (the reference's
 functions take one 1-D signal per call).
@@ -181,17 +181,23 @@ def sd(s_out, s_in, db=True):
     return 10.0 * torch.log10(r) if db else r
 
 
-def tango_scores(y, s, n, s_dry, n_dry, times, fs):
-    """The scoring block of the reference's tango.main (tango.py:541-593) without STOI, batched over utterances and
-    nodes.  y, s, n [B, K, L]: mixture, target and noise at each node's reference microphone; s_dry, n_dry [B, L_dry]
-    the dry sources of every utterance; times: the to_time() outputs ('yf', 'z_y', 'sf', 'nf', 'z_s', 'z_n', each
-    [B, K, L]); float32 CUDA tensors.  Every signal is cut to [fs:min_len] as the reference does.
+def tango_scores(y, s, n, s_dry, n_dry, times, fs, *, stoi=False):
+    """The scoring block of the reference's tango.main (tango.py:541-593), batched over utterances and nodes.
+    y, s, n [B, K, L]: mixture, target and noise at each node's reference microphone; s_dry, n_dry [B, L_dry] the dry
+    sources of every utterance; times: the to_time() outputs ('yf', 'z_y', 'sf', 'nf', 'z_s', 'z_n', each [B, K, L]);
+    float32 CUDA tensors.  Every signal is cut to [fs:min_len] as the reference does.
     Returns (results, resultsz) [B, K] float64 tensors keyed like the reference's two result pickles, without
-    'delta_stoi*' and without 'snr_in_raw' (the caller's SNRs).
+    'snr_in_raw' (the caller's SNRs), and without 'delta_stoi*' unless stoi=True.
 
     bss(refs, ests) is only read at row 0, and row 0's scores depend on no other estimate row, so only the first row
     of each estimate set is correlated: (sh, szh, y) against the node's (s, n), and the same rows of all K nodes of an
-    utterance against its dry (s_dry, n_dry), whose Gram matrix is factored once for the K nodes."""
+    utterance against its dry (s_dry, n_dry), whose Gram matrix is factored once for the K nodes.
+
+    stoi=True adds tango.py:569-578 under the reference's key names: results 'delta_stoi_cnv' = stoi(s, sh) -
+    stoi(s, y) and 'delta_stoi_dry' = stoi(s_dry, sh) - stoi(s_dry, y); resultsz 'delta_stoi' and 'delta_stoi_dry',
+    the same with szh.  The six calls of a node are six pairs of 2 cleans (s, and s_dry shared by the utterance's
+    nodes) and 3 degraded signals (y, sh, szh): each signal is resampled once and each clean's silent-frame selection
+    and band envelopes are computed once."""
     from . import bss_eval
     B, K, L = y.shape
     min_len = min(L, times["yf"].shape[-1], s_dry.shape[-1], n_dry.shape[-1])
@@ -226,4 +232,24 @@ def tango_scores(y, s, n, s_dry, n_dry, times, fs):
     resultsz = {"sar_cnv": sar[..., 1], "sir_cnv": sir[..., 1], "sdr_cnv": sdr[..., 1],
                 "snr_out": snr_out_z, "fw_sd_cnv": sd_cnv_z, "fw_sd_dry": sd_dry_z,
                 "sar_dry": d_sar[..., 1], "sir_dry": d_sir[..., 1], "sdr_dry": d_sdr[..., 1], **shared}
+    if stoi:
+        d = _tango_stoi(ss, sd_, yy, sh, szh, fs)                                # [B, K, 6]
+        results["delta_stoi_cnv"], results["delta_stoi_dry"] = d[..., 1] - d[..., 0], d[..., 4] - d[..., 3]
+        resultsz["delta_stoi"], resultsz["delta_stoi_dry"] = d[..., 2] - d[..., 0], d[..., 5] - d[..., 3]
     return results, resultsz
+
+
+def _tango_stoi(s, s_dry, y, sh, szh, fs):
+    """STOI of the six pairs of every node, [B, K, 6]: (s, y), (s, sh), (s, szh), (s_dry, y), (s_dry, sh),
+    (s_dry, szh).  s, y, sh, szh [B, K, L]; s_dry [B, L]."""
+    from . import stoi as _stoi
+    B, K, L = s.shape
+    cleans = torch.cat((s.reshape(B * K, L), s_dry.reshape(B, L)))               # node cleans, then dry cleans
+    degraded = torch.stack((y, sh, szh), dim=2).reshape(B * K * 3, L)            # [B, K, 3] rows
+    node = torch.arange(B * K, device=s.device)
+    dry = B * K + node // K
+    deg = 3 * node[:, None] + torch.arange(3, device=s.device)                   # [B K, 3]
+    cl = torch.stack((node, dry), dim=1)[:, :, None].expand(B * K, 2, 3)         # [B K, 2, 3]
+    pairs = torch.stack((cl, deg[:, None, :].expand(B * K, 2, 3)), dim=-1)       # [B K, 2, 3, 2]
+    d = _stoi.stoi_pairs(cleans.contiguous(), degraded.contiguous(), pairs.reshape(-1, 2), fs)
+    return d.view(B, K, 6)

@@ -293,6 +293,32 @@ DISCO_API size_t disco_bss_eval_workspace(int n_set, int nsrc, int n_est, int le
 DISCO_API int disco_bss_eval(const float* refs, const float* ests, double* norms, int n_set, int nsrc, int n_est,
                              int length, int flen, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- STOI (float64) -------------------------------------------------------------------------------------
+ * Classic STOI as pystoi 0.3 computes it (pystoi.stoi.stoi(x, y, fs_sig), called six times per node by the
+ * reference's evaluation, tango.py:569-578), for many (clean, degraded) pairs at once.
+ *
+ * disco_resample_poly: scipy.signal.resample_poly(x, up, down, window=taps) of n_sig rows, float32 in, float64 out.
+ *   x [n_sig][length] float32; y [n_sig][ceil(length up / down)] float64 out; taps [n_taps] float64 (scipy's `window`:
+ *   the kernel applies the gain `up` itself).  up and down >= 1 must be coprime and not both 1 (scipy returns a copy
+ *   then).  Output sample j is sum_n x[n] up taps[(j + r) down - p - n up] with scipy's centring pre-pad
+ *   p = down - h % down and r = (h + p) / down, h = (n_taps - 1) / 2.
+ *
+ * disco_stoi: STOI of 10 kHz float64 signals (resample first at any other rate).
+ *   cleans   [n_clean][length] float64, degraded [n_deg][length] float64
+ *   pairs    [n_pair][2] int32: (clean index, degraded index); an index out of range gives d = NaN, n_frames = -1
+ *   d        [n_pair] float64 out: the score, 1e-5 where fewer than 30 STFT frames remain (pystoi's value; it warns)
+ *   n_sel    [n_clean] int32 out: frames (256 samples, every 128) within 40 dB of the clean's loudest frame
+ *   n_frames [n_pair] int32 out: STFT frames scored = n_sel of the pair's clean - 1
+ * Every clean's selection and band envelopes are computed once however many pairs share it.  length >= 256 (pystoi
+ * raises below).  workspace: disco_stoi_workspace() bytes (0 for invalid sizes); it grows with n_clean + n_pair and
+ * with length: batch the pairs in chunks. */
+DISCO_API int disco_resample_poly(const float* x, double* y, const double* taps, int n_taps, int up, int down,
+                                  int n_sig, int length, void* stream);
+DISCO_API size_t disco_stoi_workspace(int n_clean, int n_pair, int length);
+DISCO_API int disco_stoi(const double* cleans, const double* degraded, const int* pairs, double* d, int* n_sel,
+                         int* n_frames, int n_clean, int n_deg, int n_pair, int length, void* workspace,
+                         size_t workspace_bytes, void* stream);
+
 /* ---- layout helpers -------------------------------------------------------------------------------
  * out[b][c][r] = in[b][r][c] for `batch` planes (complex64 / float32).  Used at the Python
  * boundary to move between the reference (F, T) layout and the native (T, F) layout. */

@@ -43,3 +43,15 @@ for (B, K, C, n_fft, block, sizes) in ((3, 1, 3, 256, 4, (100, 0, 700, 1, 2500))
 x = torch.randn(37, 3000, device=dev)
 print("ok bank", float(post.fw_snr(x[:, 100:], 0.5 * torch.randn(37, 2900, device=dev), 16000)[1].mean()))
 torch.cuda.synchronize()
+# STOI: resampler, silent-frame selection (one all-silent clean), bands of cleans and pairs, a short pair (1e-5)
+import warnings
+from disco_b200 import stoi
+x = torch.randn(3, 24000, device=dev) * (torch.arange(24000, device=dev) % 8000 < 5000)
+x[1] = 0
+with warnings.catch_warnings():
+    warnings.simplefilter("ignore", RuntimeWarning)
+    d = stoi.stoi_pairs(x, torch.cat((x + 0.3 * torch.randn_like(x), x[:, :5000].repeat(1, 5)[:, :24000])),
+                        [(0, 0), (1, 1), (2, 2), (0, 3), (2, 5)], 16000)
+    d_short = stoi.stoi(x[:, :3000], x[:, :3000], 16000)
+torch.cuda.synchronize()
+print("ok stoi", d.tolist(), d_short.tolist())
