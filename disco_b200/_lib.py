@@ -54,6 +54,8 @@ SIGNATURES = {
     "disco_filter_sum": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                                  c_int, c_int, c_int, c_int_p, c_int, c_int, c_void_p]),
     "disco_istft": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "disco_stft_lengths": (c_int, [c_void_p, c_void_p, c_int_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "disco_istft_lengths": (c_int, [c_void_p, c_void_p, c_int_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "disco_scm_recursive": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, ctypes.c_double,
                                     c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int_p, c_int, c_void_p]),
     "disco_filter_sum_blocks": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
@@ -68,6 +70,10 @@ SIGNATURES = {
     "disco_bss_eval": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_size_t,
                                c_void_p]),
     "disco_resample_poly": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "disco_resample_poly_lengths": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p,
+                                            c_int_p, c_void_p]),
+    "disco_stoi_lengths": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
+                                   c_int, c_void_p, c_int_p, c_void_p, c_size_t, c_void_p]),
     "disco_stoi_workspace": (c_size_t, [c_int, c_int, c_int]),
     "disco_stoi": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                            c_void_p, c_size_t, c_void_p]),

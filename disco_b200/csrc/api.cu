@@ -504,6 +504,66 @@ int disco_istft(const void* Y, float* x, int n_sig, int T, int length, int n_fft
     return 0;
 }
 
+// the per-signal lengths of disco_stft_lengths / disco_istft_lengths: lo < lengths[s] <= hi for every signal
+static int check_lengths(const int* lengths_host, int n_sig, int lo, int hi) {
+    if (!lengths_host) return fail(DISCO_ERR_INVALID, "null pointer");
+    for (int s = 0; s < n_sig; ++s)
+        if (lengths_host[s] <= lo || lengths_host[s] > hi)
+            return fail(DISCO_ERR_INVALID, "a length is out of range (too short, or longer than the rows)");
+    return 0;
+}
+
+int disco_stft_lengths(const float* x, const int* lengths, const int* lengths_host, void* Y, int n_sig, int length,
+                       int n_fft, void* stream) {
+    if (!valid_nfft(n_fft)) return fail(DISCO_ERR_INVALID, "n_fft must be 256, 512 or 1024");
+    if (n_sig <= 0 || length <= n_fft / 2)
+        return fail(DISCO_ERR_INVALID, "need n_sig > 0 and length > n_fft/2 (reflect padding)");
+    int rc = check_lengths(lengths_host, n_sig, n_fft / 2, length);
+    if (rc) return rc;
+    if (!x || !lengths || !Y) return fail(DISCO_ERR_INVALID, "null pointer");
+    Tables tb;
+    rc = get_tables(n_fft, &tb);
+    if (rc) return rc;
+    StftLengthsArgs a;
+    memset(&a, 0, sizeof(a));
+    a.x = x;
+    a.lengths = lengths;
+    a.Y = (float2*)Y;
+    a.twiddle = tb.twiddle;
+    a.window = tb.win_half;
+    a.n_sig = n_sig;
+    a.L = length;
+    a.T = disco_n_frames(length, n_fft);
+    CU(launch_stft_lengths(a, n_fft, (cudaStream_t)stream), "stft_lengths launch");
+    return 0;
+}
+
+int disco_istft_lengths(const void* Y, const int* lengths, const int* lengths_host, float* x, int n_sig, int T,
+                        int length, int n_fft, void* stream) {
+    if (!valid_nfft(n_fft)) return fail(DISCO_ERR_INVALID, "n_fft must be 256, 512 or 1024");
+    if (n_sig <= 0 || T < 1 || length < 1) return fail(DISCO_ERR_INVALID, "bad arguments");
+    int rc = check_lengths(lengths_host, n_sig, 0, length);
+    if (rc) return rc;
+    if (!Y || !lengths || !x) return fail(DISCO_ERR_INVALID, "null pointer");
+    Tables tb;
+    rc = get_tables(n_fft, &tb);
+    if (rc) return rc;
+    IstftArgs a;
+    memset(&a, 0, sizeof(a));
+    a.Y = (const float2*)Y;
+    a.x = x;
+    a.twiddle = tb.twiddle;
+    a.window = tb.win;
+    a.n_sig = n_sig;
+    a.L = length;
+    a.y_frames = T;
+    a.ld = length;
+    a.j_end = T;
+    a.tail = 1;
+    CU(launch_istft_lengths(a, lengths, n_fft, (cudaStream_t)stream), "istft_lengths launch");
+    return 0;
+}
+
 int disco_scm_recursive(const void* Y, const void* Z, const float* mask, const void* R0ss, const void* R0nn, void* Rss,
                         void* Rnn, double lambda_cor, int block, int weight_power, int n_utt, int K, int C, int T,
                         int n_fft, const int* node_sel, int n_sel, void* stream) {
@@ -699,8 +759,8 @@ int disco_bss_eval(const float* refs, const float* ests, double* norms, int n_se
 
 static long long gcd_ll(long long a, long long b) { return b == 0 ? a : gcd_ll(b, a % b); }
 
-int disco_resample_poly(const float* x, double* y, const double* taps, int n_taps, int up, int down, int n_sig,
-                        int length, void* stream) {
+static int resample_common(const float* x, double* y, const double* taps, int n_taps, int up, int down, int n_sig,
+                           int length, const int* lengths, void* stream) {
     if (n_taps < 1 || up < 1 || down < 1 || n_sig < 1 || length < 1) return fail(DISCO_ERR_INVALID, "bad sizes");
     if (gcd_ll(up, down) != 1 || (up == 1 && down == 1))
         return fail(DISCO_ERR_INVALID, "up and down must be coprime and not both 1");
@@ -712,6 +772,7 @@ int disco_resample_poly(const float* x, double* y, const double* taps, int n_tap
     a.x = x;
     a.y = y;
     a.taps = taps;
+    a.lengths = lengths;
     a.n_taps = n_taps;
     a.up = up;
     a.down = down;
@@ -720,6 +781,20 @@ int disco_resample_poly(const float* x, double* y, const double* taps, int n_tap
     a.n_out = (int)n_out;
     CU(launch_resample_poly(a, (cudaStream_t)stream), "resample_poly launch");
     return 0;
+}
+
+int disco_resample_poly(const float* x, double* y, const double* taps, int n_taps, int up, int down, int n_sig,
+                        int length, void* stream) {
+    return resample_common(x, y, taps, n_taps, up, down, n_sig, length, nullptr, stream);
+}
+
+int disco_resample_poly_lengths(const float* x, double* y, const double* taps, int n_taps, int up, int down, int n_sig,
+                                int length, const int* lengths, const int* lengths_host, void* stream) {
+    if (n_sig < 1 || length < 1) return fail(DISCO_ERR_INVALID, "bad sizes");
+    int rc = check_lengths(lengths_host, n_sig, 0, length);
+    if (rc) return rc;
+    if (!lengths) return fail(DISCO_ERR_INVALID, "null pointer");
+    return resample_common(x, y, taps, n_taps, up, down, n_sig, length, lengths, stream);
 }
 
 static int stoi_check(int n_clean, int n_deg, int n_pair, int length) {
@@ -736,8 +811,9 @@ size_t disco_stoi_workspace(int n_clean, int n_pair, int length) {
     return stoi_ws_bytes(n_clean, n_pair, length);
 }
 
-int disco_stoi(const double* cleans, const double* degraded, const int* pairs, double* d, int* n_sel, int* n_frames,
-               int n_clean, int n_deg, int n_pair, int length, void* workspace, size_t workspace_bytes, void* stream) {
+static int stoi_common(const double* cleans, const double* degraded, const int* pairs, double* d, int* n_sel,
+                       int* n_frames, int n_clean, int n_deg, int n_pair, int length, const int* lengths,
+                       void* workspace, size_t workspace_bytes, void* stream) {
     int rc = stoi_check(n_clean, n_deg, n_pair, length);
     if (rc) return rc;
     if (!cleans || !degraded || !pairs || !d || !n_sel || !n_frames) return fail(DISCO_ERR_INVALID, "null pointer");
@@ -752,12 +828,31 @@ int disco_stoi(const double* cleans, const double* degraded, const int* pairs, d
     a.n_sel = n_sel;
     a.n_frames = n_frames;
     a.energy = (double*)workspace;
+    a.lengths = lengths;
     a.n_clean = n_clean;
     a.n_deg = n_deg;
     a.n_pair = n_pair;
     a.L = length;
     CU(launch_stoi(a, (cudaStream_t)stream), "stoi launch");
     return 0;
+}
+
+int disco_stoi(const double* cleans, const double* degraded, const int* pairs, double* d, int* n_sel, int* n_frames,
+               int n_clean, int n_deg, int n_pair, int length, void* workspace, size_t workspace_bytes, void* stream) {
+    return stoi_common(cleans, degraded, pairs, d, n_sel, n_frames, n_clean, n_deg, n_pair, length, nullptr, workspace,
+                       workspace_bytes, stream);
+}
+
+int disco_stoi_lengths(const double* cleans, const double* degraded, const int* pairs, double* d, int* n_sel,
+                       int* n_frames, int n_clean, int n_deg, int n_pair, int length, const int* lengths,
+                       const int* lengths_host, void* workspace, size_t workspace_bytes, void* stream) {
+    int rc = stoi_check(n_clean, n_deg, n_pair, length);
+    if (rc) return rc;
+    rc = check_lengths(lengths_host, n_clean, kStoiFrame - 1, length);
+    if (rc) return rc;
+    if (!lengths) return fail(DISCO_ERR_INVALID, "null pointer");
+    return stoi_common(cleans, degraded, pairs, d, n_sel, n_frames, n_clean, n_deg, n_pair, length, lengths, workspace,
+                       workspace_bytes, stream);
 }
 
 int disco_transpose_c64(const void* in, void* out, int batch, int rows, int cols, void* stream) {

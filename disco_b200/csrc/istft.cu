@@ -181,6 +181,53 @@ __global__ void __launch_bounds__(IGeom<N>::THREADS) stream_istft_kernel(IstftAr
     istft_body<N, true>(p);
 }
 
+// Whole signals of their own lengths (disco_istft_lengths, launched from lengths.cu): signal s is the iSTFT of its
+// frames [0, min(j_end, 1 + lengths[s] / H)) cut to lengths[s] samples, exactly as disco_istft runs it on those frames
+// and that length, and is zero from lengths[s] to L (the row length).  A pair of equal lengths runs as a pair, as
+// disco_istft pairs it; the two signals of a pair of different lengths run one after the other, each alone.
+template <int N>
+__global__ void __launch_bounds__(IGeom<N>::THREADS) istft_lengths_kernel(IstftArgs p, const int* lengths) {
+    constexpr int H = IGeom<N>::H, F = IGeom<N>::F;
+    const int sa = 2 * blockIdx.y, sb = sa + 1;
+    const bool has_b = sb < p.n_sig;
+    const int La = lengths[sa], Lb = has_b ? lengths[sb] : La;
+    // s0: the signal the body sees as the pair's first; alone: no partner
+    auto run = [&](int s0, bool alone, int len) {
+        IstftArgs q = p;
+        q.L = len;
+        q.j_end = min(p.j_end, 1 + len / H);
+        if ((int)blockIdx.x * p.fpc >= q.j_end) return;   // CTA-uniform: this chunk lies past the signal's frames
+        if (alone) {
+            q.Y = p.Y + (ptrdiff_t)(s0 - sa) * p.y_frames * F;
+            q.x = p.x + (ptrdiff_t)(s0 - sa) * p.ld;
+            q.n_sig = sa + 1;
+        }
+        istft_body<N, false>(q);
+    };
+    if (La == Lb) {
+        run(sa, false, La);
+    } else {
+        run(sa, true, La);
+        __syncthreads();   // the second run reloads the shared tables and the carry
+        run(sb, true, Lb);
+    }
+    if (blockIdx.x == 0) {
+        for (int s = La + threadIdx.x; s < p.L; s += blockDim.x) p.x[(size_t)sa * p.ld + s] = 0.f;
+        if (has_b)
+            for (int s = Lb + threadIdx.x; s < p.L; s += blockDim.x) p.x[(size_t)sb * p.ld + s] = 0.f;
+    }
+}
+
+IstftLengthsKernel istft_lengths_kernel_for(int n_fft) {
+    switch (n_fft) {
+        case 256: return {(const void*)istft_lengths_kernel<256>, IGeom<256>::THREADS, IGeom<256>::SMEM, IGeom<256>::ITEMS};
+        case 512: return {(const void*)istft_lengths_kernel<512>, IGeom<512>::THREADS, IGeom<512>::SMEM, IGeom<512>::ITEMS};
+        case 1024: return {(const void*)istft_lengths_kernel<1024>, IGeom<1024>::THREADS, IGeom<1024>::SMEM,
+                           IGeom<1024>::ITEMS};
+        default: return {nullptr, 0, 0, 0};
+    }
+}
+
 template <int N>
 static cudaError_t launch_n(IstftArgs a, cudaStream_t st) {
     using G = IGeom<N>;

@@ -239,6 +239,8 @@ struct ResampleArgs {
     const float* x;      // [n_sig][n_in]
     double* y;           // [n_sig][n_out], n_out = ceil(n_in up / down)
     const double* taps;  // [n_taps] scipy's `window` (the gain `up` is applied in the kernel, as scipy does)
+    const int* lengths;  // null, or [n_sig]: signal s is its first lengths[s] <= n_in samples (zero output after
+                         // ceil(lengths[s] up / down))
     int n_taps, up, down, n_sig, n_in, n_out;
 };
 cudaError_t launch_resample_poly(const ResampleArgs& a, cudaStream_t st);
@@ -257,6 +259,8 @@ struct StoiArgs {
     double* energy;          // workspace [n_clean][n_fr]
     int* sel;                // workspace [n_clean][n_fr]: kept frame indices, in order
     double* tob;             // workspace [n_clean + n_pair][n_fr][kStoiBands]: band envelopes
+    const int* lengths;      // null, or [n_clean]: clean c (and every degraded signal paired with it) is its first
+                             // lengths[c] <= L samples; its frame selection stops at the last full frame of those
     int n_clean, n_deg, n_pair, L, n_fr;
 };
 int stoi_n_fr(int L);
@@ -280,6 +284,28 @@ struct IstftArgs {
     int tail;               // 1: also block j_end (second half of frame j_end - 1) and the zero fill up to L
 };
 cudaError_t launch_istft(const IstftArgs& a, int n_fft, cudaStream_t st);
+
+// Signals of their own lengths in rows of a common length (lengths.cu).  Signal s holds lengths[s] samples
+// (hop < lengths[s] <= L) and 1 + lengths[s] / hop frames; the rest of its row (samples, frames) is zero.
+struct StftLengthsArgs {
+    const float* x;         // [n_sig][L] float32
+    const int* lengths;     // [n_sig] device
+    float2* Y;              // [n_sig][T][F], T = 1 + L / hop
+    const float2* twiddle;  // [N/32][32]
+    const float* window;    // [N]: 0.5 * periodic Hann
+    int n_sig, L, T;
+};
+cudaError_t launch_stft_lengths(const StftLengthsArgs& a, int n_fft, cudaStream_t st);
+// a: as disco_istft fills it (Y [n_sig][y_frames][F], x [n_sig][L], j_end = y_frames); lengths [n_sig] device
+cudaError_t launch_istft_lengths(const IstftArgs& a, const int* lengths, int n_fft, cudaStream_t st);
+// istft.cu's per-length kernel (it runs istft_body) and its launch geometry, for launch_istft_lengths
+struct IstftLengthsKernel {
+    const void* fn;
+    int threads;
+    size_t smem;
+    int items;
+};
+IstftLengthsKernel istft_lengths_kernel_for(int n_fft);
 
 // Streaming STFT (stream.cu): disco_stft on a signal that arrives chunk by chunk.
 struct StreamStftArgs {

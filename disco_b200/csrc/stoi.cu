@@ -35,18 +35,26 @@ __constant__ int kStoiEdges[kStoiBands + 1] = {7, 9, 11, 14, 17, 22, 27, 34, 43,
 // np.hanning(258)[1:-1][n] = 0.5 + 0.5 cos(pi (2 n - 255) / 257)
 __device__ __forceinline__ double stoi_hann(int n) { return 0.5 + 0.5 * cospi((double)(2 * n - 255) / 257.0); }
 
+__host__ __device__ __forceinline__ int stoi_frames(int L) { return L < kStoiFrame ? 0 : (L - kStoiFrame) / kHop + 1; }
+
 __device__ __forceinline__ long long floor_div(long long a, long long b) { return a >= 0 ? a / b : -((-a + b - 1) / b); }
 
 __global__ void __launch_bounds__(256) resample_poly_kernel(ResampleArgs a, int blocks_per_sig) {
     const int sig = blockIdx.x / blocks_per_sig;
     const long long j = (long long)(blockIdx.x % blocks_per_sig) * blockDim.x + threadIdx.x;
     if (j >= a.n_out) return;
+    // a signal of its own length n_in_s <= n_in: output samples from ceil(n_in_s up / down) on are 0
+    const long long n_in_s = a.lengths ? a.lengths[sig] : a.n_in;
+    if (a.lengths && j >= (n_in_s * a.up + a.down - 1) / a.down) {
+        a.y[(size_t)sig * a.n_out + j] = 0.0;
+        return;
+    }
     const int half = (a.n_taps - 1) / 2;
     const int pre_pad = a.down - half % a.down;
     const int pre_remove = (half + pre_pad) / a.down;
     const long long t = (j + pre_remove) * a.down - pre_pad;    // tap index of x[0]; x[n] meets tap t - n up
     const long long n_lo = max(floor_div(t - a.n_taps + a.up, a.up), 0LL);
-    const long long n_hi = min(floor_div(t, a.up), (long long)a.n_in - 1);
+    const long long n_hi = min(floor_div(t, a.up), n_in_s - 1);
     const float* x = a.x + (size_t)sig * a.n_in;
     double acc = 0.0;
     for (long long n = n_lo; n <= n_hi; ++n) acc = fma((double)__ldg(x + n), __ldg(a.taps + (t - n * a.up)) * a.up, acc);
@@ -66,8 +74,10 @@ __global__ void __launch_bounds__(kSelThreads) stoi_select_kernel(StoiArgs a) {
     const double* x = a.cleans + (size_t)c * a.L;
     double* e = a.energy + (size_t)c * a.n_fr;
     int* sel = a.sel + (size_t)c * a.n_fr;
+    // frames of this clean: pystoi's framing of the clean trimmed to its own length stops at its last full frame
+    const int n_fr = a.lengths ? stoi_frames(a.lengths[c]) : a.n_fr;
     double mx = -INFINITY;
-    for (int f = warp; f < a.n_fr; f += kSelWarps) {
+    for (int f = warp; f < n_fr; f += kSelWarps) {
         const double* fr = x + (size_t)f * kHop;
         double s = 0.0;
         for (int r = lane; r < kStoiFrame; r += 32) {
@@ -86,9 +96,9 @@ __global__ void __launch_bounds__(kSelThreads) stoi_select_kernel(StoiArgs a) {
     for (int w = 1; w < kSelWarps; ++w) emax = fmax(emax, wmax[w]);
     const double thr = emax - kDynRange;
     int base = 0;
-    for (int f0 = 0; f0 < a.n_fr; f0 += kSelThreads) {
+    for (int f0 = 0; f0 < n_fr; f0 += kSelThreads) {
         const int f = f0 + tid;
-        const bool keep = f < a.n_fr && thr - e[f] < 0.0;
+        const bool keep = f < n_fr && thr - e[f] < 0.0;
         const unsigned b = __ballot_sync(0xffffffffu, keep);
         if (lane == 0) cnt[warp] = __popc(b);
         __syncthreads();
@@ -252,7 +262,7 @@ cudaError_t launch_resample_poly(const ResampleArgs& a, cudaStream_t st) {
     return cudaGetLastError();
 }
 
-int stoi_n_fr(int L) { return L < kStoiFrame ? 0 : (L - kStoiFrame) / kHop + 1; }
+int stoi_n_fr(int L) { return stoi_frames(L); }
 
 size_t stoi_ws_bytes(int n_clean, int n_pair, int L) {
     const size_t n_fr = (size_t)stoi_n_fr(L);

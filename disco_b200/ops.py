@@ -8,6 +8,7 @@ reference's NumPy layout ``[..., F, T]`` for masks / final outputs (SURVEY.md §
 import ctypes
 import math
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -429,6 +430,67 @@ def istft(Y, length, n_fft=512):
     return x
 
 
+def signal_lengths(lengths, lead, L, lo=0):
+    """Per-signal lengths of a batch [*lead, L]: `lengths` (sequence, NumPy array or tensor of integers) covers the
+    leading axes lead[:m] and is repeated over the rest (e.g. one length per utterance of [B, K, C, L]).  Every
+    length must satisfy lo < length <= L.  Returns the flattened lengths as a host int32 NumPy array."""
+    import numpy as np
+    if isinstance(lengths, torch.Tensor):
+        if lengths.is_floating_point() or lengths.is_complex():
+            raise TypeError("lengths must be integers, got %s" % lengths.dtype)
+        lengths = lengths.detach().cpu().numpy()
+    arr = np.asarray(lengths)
+    if arr.dtype.kind not in "iu":
+        raise TypeError("lengths must be integers, got %s" % arr.dtype)
+    lead = tuple(int(v) for v in lead)
+    if arr.ndim > len(lead) or tuple(arr.shape) != lead[:arr.ndim]:
+        raise ValueError("lengths shape %s does not match the leading axes %s" % (tuple(arr.shape), lead))
+    if arr.size and (int(arr.min()) <= lo or int(arr.max()) > L):
+        raise ValueError("every length must lie in (%d, %d]" % (lo, L))
+    full = np.broadcast_to(arr.reshape(arr.shape + (1,) * (len(lead) - arr.ndim)), lead)
+    return np.ascontiguousarray(full, dtype=np.int32).reshape(-1)
+
+
+def _lengths_args(host, device):
+    """(device int32 tensor, ctypes pointer to the host copy) of host lengths."""
+    host = np.require(host, dtype=np.int32, requirements=("C", "W"))
+    return (torch.from_numpy(host).to(device), host.ctypes.data_as(_lib.c_int_p))
+
+
+@_on_device
+def stft_lengths(x, lengths, n_fft=512):
+    """x [..., L] float32, signals of their own lengths (zero after) -> Y [..., T, F] complex64, T = 1 + L // hop.
+    lengths: per signal, or per leading index repeated over the remaining axes (see signal_lengths); every length in
+    (n_fft / 2, L].  Frame t < 1 + length // hop of a signal is stft() of the signal trimmed to its length (reflect
+    padding at its own end); later frames are 0."""
+    _need(x, torch.float32, "x")
+    L = x.shape[-1]
+    n_sig = x.numel() // L
+    host = signal_lengths(lengths, x.shape[:-1], L, lo=n_fft // 2)
+    T, F = n_frames(L, n_fft), n_fft // 2 + 1
+    Y = torch.empty(x.shape[:-1] + (T, F), dtype=torch.complex64, device=x.device)
+    dev, hp = _lengths_args(host, x.device)
+    _lib.check(_lib.load().disco_stft_lengths(_ptr(x), _ptr(dev), hp, _ptr(Y), n_sig, L, n_fft, _stream()))
+    return Y
+
+
+@_on_device
+def istft_lengths(Y, lengths, length, n_fft=512):
+    """Y [..., T, F] complex64 -> x [..., length] float32, each signal of its own length: samples < lengths[s] are
+    istft(Y_s[:1 + lengths[s] // hop], lengths[s]), the rest 0.  lengths as in stft_lengths, each in (0, length]."""
+    _need(Y, torch.complex64, "Y")
+    T, F = Y.shape[-2:]
+    if F != n_fft // 2 + 1:
+        raise ValueError("last dimension must be n_fft/2 + 1 bins")
+    n_sig = Y.numel() // (T * F)
+    host = signal_lengths(lengths, Y.shape[:-2], int(length))
+    x = torch.empty(Y.shape[:-2] + (int(length),), dtype=torch.float32, device=Y.device)
+    dev, hp = _lengths_args(host, Y.device)
+    _lib.check(_lib.load().disco_istft_lengths(_ptr(Y), _ptr(dev), hp, _ptr(x), n_sig, T, int(length), n_fft,
+                                               _stream()))
+    return x
+
+
 @_on_device
 def scm_recursive(Y, mask, Z=None, lambda_cor=0.95, block=8, power=2, R0=None, n_fft=512, node_sel=None):
     """Exponentially smoothed SCM pair, R <- lambda R + (1 - lambda) w x x^H per frame (reference
@@ -609,10 +671,12 @@ def bss_eval(refs, ests, flen=512):
 
 
 @_on_device
-def resample_poly(x, taps, up, down):
+def resample_poly(x, taps, up, down, lengths=None):
     """scipy.signal.resample_poly(x, up, down, window=taps) along the last axis (disco_resample_poly).
     x [..., L] float32, taps [n] float64 (scipy's `window`; the gain `up` is applied inside) -> [..., ceil(L up / down)]
-    float64.  up and down are reduced by their gcd first, as scipy does; equal rates return x as float64."""
+    float64.  up and down are reduced by their gcd first, as scipy does; equal rates return x as float64.
+    lengths (per signal, or per leading index as in signal_lengths; each in (0, L]): row s is its first lengths[s]
+    samples, and its output is resample_poly of that trimmed row followed by zeros (disco_resample_poly_lengths)."""
     _need(x, torch.float32, "x")
     _need(taps, torch.float64, "taps")
     up, down = int(up), int(down)
@@ -620,16 +684,22 @@ def resample_poly(x, taps, up, down):
         raise ValueError("up and down must be >= 1")
     g = math.gcd(up, down)
     up, down = up // g, down // g
-    if up == down == 1:
-        return x.double()
     L = x.shape[-1]
+    host = None if lengths is None else signal_lengths(lengths, x.shape[:-1], L)
+    if up == down == 1:
+        return x.double()    # rows are zero after their lengths already
     n_out = -(-L * up // down)
     y = torch.empty(x.shape[:-1] + (n_out,), dtype=torch.float64, device=x.device)
     n_sig = x.numel() // L if L else 0
     if n_sig == 0:
         return y
-    _lib.check(_lib.load().disco_resample_poly(_ptr(x), _ptr(y), _ptr(taps), taps.numel(), up, down, n_sig, L,
-                                               _stream()))
+    if host is None:
+        _lib.check(_lib.load().disco_resample_poly(_ptr(x), _ptr(y), _ptr(taps), taps.numel(), up, down, n_sig, L,
+                                                   _stream()))
+    else:
+        dev, hp = _lengths_args(host, x.device)
+        _lib.check(_lib.load().disco_resample_poly_lengths(_ptr(x), _ptr(y), _ptr(taps), taps.numel(), up, down, n_sig,
+                                                           L, _ptr(dev), hp, _stream()))
     return y
 
 
@@ -639,12 +709,13 @@ STOI_WORKSPACE_CAP = 1 << 30
 
 
 @_on_device
-def stoi(cleans, degraded, pairs):
+def stoi(cleans, degraded, pairs, lengths=None):
     """Classic STOI of 10 kHz signals (disco_stoi).  cleans [C, L], degraded [D, L] float64, pairs [P, 2] int32
     (clean index, degraded index) -> d [P] float64 (1e-5 below 30 STFT frames), n_sel [C] int32 (frames kept by the
     silent-frame removal; -1 for a clean no pair names), n_frames [P] int32 (STFT frames scored).  Pairs are processed
     in chunks whose workspace stays within STOI_WORKSPACE_CAP bytes (one pair at least); a chunk computes only the
-    cleans its pairs name, each once."""
+    cleans its pairs name, each once.  lengths [C] (each in [256, L], or None): clean c and every degraded signal
+    paired with it are their first lengths[c] samples (disco_stoi_lengths); None scores whole rows."""
     _need(cleans, torch.float64, "cleans")
     _need(degraded, torch.float64, "degraded")
     _need(pairs, torch.int32, "pairs")
@@ -666,14 +737,25 @@ def stoi(cleans, degraded, pairs):
             int(pairs[:, 1].min()) < 0 or int(pairs[:, 1].max()) >= D:
         raise IndexError("stoi: pair indices out of range (%d cleans, %d degraded signals)" % (C, D))
     lib = _lib.load()
+    host = None if lengths is None else signal_lengths(lengths, (C,), L, lo=255)
+
+    def run(cl, pr, d_out, sel_out, nf_out, n_cl, n_pr, ws, ws_bytes, hl):
+        if hl is None:
+            _lib.check(lib.disco_stoi(_ptr(cl), _ptr(degraded), _ptr(pr), _ptr(d_out), _ptr(sel_out), _ptr(nf_out),
+                                      n_cl, D, n_pr, L, _ptr(ws), ws_bytes, _stream()))
+        else:
+            ld, hp = _lengths_args(hl, dev)
+            _lib.check(lib.disco_stoi_lengths(_ptr(cl), _ptr(degraded), _ptr(pr), _ptr(d_out), _ptr(sel_out),
+                                              _ptr(nf_out), n_cl, D, n_pr, L, _ptr(ld), hp, _ptr(ws), ws_bytes,
+                                              _stream()))
+
     per_pair = lib.disco_stoi_workspace(1, 1, L)
     if per_pair == 0:
         _lib.check(lib.disco_stoi(None, None, None, None, None, None, 1, 1, 1, L, None, 0, _stream()))
     if lib.disco_stoi_workspace(C, P, L) <= STOI_WORKSPACE_CAP:
         ws_bytes = lib.disco_stoi_workspace(C, P, L)
         ws = torch.empty(ws_bytes // 8 + 1, dtype=torch.float64, device=dev)
-        _lib.check(lib.disco_stoi(_ptr(cleans), _ptr(degraded), _ptr(pairs), _ptr(d), _ptr(n_sel), _ptr(n_frames), C,
-                                  D, P, L, _ptr(ws), ws_bytes, _stream()))
+        run(cleans, pairs, d, n_sel, n_frames, C, P, ws, ws_bytes, host)
         named = torch.zeros(C, dtype=torch.bool, device=dev)
         named[pairs[:, 0].long()] = True
         return d, n_sel.masked_fill_(~named, -1), n_frames
@@ -686,8 +768,8 @@ def stoi(cleans, degraded, pairs):
         sub = cleans.index_select(0, used)
         pr = torch.stack((local.to(torch.int32), pairs[p0:p0 + n, 1]), dim=1).contiguous()
         sel = torch.empty(used.numel(), dtype=torch.int32, device=dev)
-        _lib.check(lib.disco_stoi(_ptr(sub), _ptr(degraded), _ptr(pr), _ptr(d[p0:]), _ptr(sel), _ptr(n_frames[p0:]),
-                                  used.numel(), D, n, L, _ptr(ws), ws_bytes, _stream()))
+        hl = None if host is None else np.ascontiguousarray(host[used.cpu().numpy()])
+        run(sub, pr, d[p0:], sel, n_frames[p0:], used.numel(), n, ws, ws_bytes, hl)
         n_sel[used] = sel
     return d, n_sel, n_frames
 

@@ -28,9 +28,11 @@ _F_NARROW = np.array([200, 250, 315, 400, 500, 630, 800, 1000, 1250, 1600, 2000,
 _G_OCTAVE = 10.0 ** 0.3          # IEC 61260-1:2014 octave ratio (what acoustics.signal.OctaveBand implements)
 
 
-def to_time(outputs, length, n_fft=512, names=("yf", "z_y", "sf", "nf", "z_s", "z_n"), layout="FT"):
+def to_time(outputs, length, n_fft=512, names=("yf", "z_y", "sf", "nf", "z_s", "z_n"), layout="FT", lengths=None):
     """outputs: dict from tango_batched ([B, K, F, T] for layout 'FT', [B, K, T, F] for 'TF').
-    Returns {name: [B, K, length] float32} for the names present (tango.py:526-539)."""
+    Returns {name: [B, K, length] float32} for the names present (tango.py:526-539).
+    lengths [B] (the tango_batched argument): utterance b is the iSTFT of its frames [0, 1 + lengths[b] // hop) to
+    lengths[b] samples, zero after them (ops.istft_lengths); None: every utterance is `length` samples long."""
     present = [n for n in names if n in outputs]
     if not present:
         return {}
@@ -39,7 +41,11 @@ def to_time(outputs, length, n_fft=512, names=("yf", "z_y", "sf", "nf", "z_s", "
         S = outputs[n]
         specs.append(ops.transpose_last2(S.contiguous()) if layout == "FT" else S)
     stack = torch.stack(specs).contiguous()                    # [n, B, K, T, F]
-    x = ops.istft(stack, int(length), n_fft)                   # [n, B, K, length]
+    if lengths is None:
+        x = ops.istft(stack, int(length), n_fft)               # [n, B, K, length]
+    else:
+        per_utt = ops.signal_lengths(lengths, stack.shape[1:2], int(length))
+        x = ops.istft_lengths(stack, np.broadcast_to(per_utt, (len(present),) + per_utt.shape), int(length), n_fft)
     return {n: x[i] for i, n in enumerate(present)}
 
 
@@ -142,10 +148,12 @@ def fw_snr(s, n, fs, vad_tar=None, vad_noi=None, clipping=1, db=True):
     return fq, mean, F
 
 
-def fw_sd(s_out, s_in, fs, clipping=1, db=True):
-    """Frequency-weighted speech distortion (reference metrics.py:211-279).  Returns (fqwt_sd, fw_sd_mean, F)."""
+def fw_sd(s_out, s_in, fs, clipping=1, db=True, *, sel_out=None, sel_in=None):
+    """Frequency-weighted speech distortion (reference metrics.py:211-279).  Returns (fqwt_sd, fw_sd_mean, F).
+    sel_out / sel_in (like s_out, or None): band statistics of that signal over its samples with sel != 0 only (as
+    fw_snr's vad_tar / vad_noi)."""
     F, w, _ = _bank(fs, 4, s_out.device)
-    sd_var = band_powers_db(s_in, fs, 4) - band_powers_db(s_out, fs, 4)
+    sd_var = band_powers_db(s_in, fs, 4, sel_in) - band_powers_db(s_out, fs, 4, sel_out)
     if clipping:
         sd_var = sd_var.clamp(0.0, 25.0)
     fq = w * sd_var
@@ -181,7 +189,7 @@ def sd(s_out, s_in, db=True):
     return 10.0 * torch.log10(r) if db else r
 
 
-def tango_scores(y, s, n, s_dry, n_dry, times, fs, *, stoi=False):
+def tango_scores(y, s, n, s_dry, n_dry, times, fs, *, stoi=False, lengths=None):
     """The scoring block of the reference's tango.main (tango.py:541-593), batched over utterances and nodes.
     y, s, n [B, K, L]: mixture, target and noise at each node's reference microphone; s_dry, n_dry [B, L_dry] the dry
     sources of every utterance; times: the to_time() outputs ('yf', 'z_y', 'sf', 'nf', 'z_s', 'z_n', each [B, K, L]);
@@ -197,11 +205,27 @@ def tango_scores(y, s, n, s_dry, n_dry, times, fs, *, stoi=False):
     stoi(s, y) and 'delta_stoi_dry' = stoi(s_dry, sh) - stoi(s_dry, y); resultsz 'delta_stoi' and 'delta_stoi_dry',
     the same with szh.  The six calls of a node are six pairs of 2 cleans (s, and s_dry shared by the utterance's
     nodes) and 3 degraded signals (y, sh, szh): each signal is resampled once and each clean's silent-frame selection
-    and band envelopes are computed once."""
+    and band envelopes are computed once.
+
+    lengths [B] (the tango_batched / to_time argument, or None): utterance b is scored over [fs, min(lengths[b],
+    min_len)), as tango_scores scores that utterance alone, trimmed.  Every signal of the utterance is taken as zero
+    after that.  BSS-eval and STOI see the zero-padded rows (trailing zeros change no projection norm; STOI's frame
+    selection stops at each utterance's own last frame); fw_snr / fw_sd filter whole rows, which does not change the
+    causal filter outputs before the end, and take their band statistics over the samples before it."""
     from . import bss_eval
     B, K, L = y.shape
     min_len = min(L, times["yf"].shape[-1], s_dry.shape[-1], n_dry.shape[-1])
-    cut = lambda x: x[..., fs:min_len]
+    keep = None
+    if lengths is None:
+        cut = lambda x: x[..., fs:min_len]
+    else:
+        lb = np.minimum(ops.signal_lengths(lengths, (B,), L), min_len) - fs            # samples scored per utterance
+        if int(lb.min()) < 1:
+            raise ValueError("tango_scores: an utterance ends before the first second (fs samples) it skips")
+        Ls = min_len - fs
+        keep = torch.arange(Ls, device=y.device)[None, :] < torch.from_numpy(lb).to(y.device)[:, None]    # [B, Ls]
+        tail = lambda x: (~keep).view((B,) + (1,) * (x.dim() - 2) + (Ls,))
+        cut = lambda x: x[..., fs:min_len].masked_fill(tail(x), 0.0)
     sh, szh, yy = cut(times["yf"]), cut(times["z_y"]), cut(y)
     sf, nf, szf, nzf = cut(times["sf"]), cut(times["nf"]), cut(times["z_s"]), cut(times["z_n"])
     ss, nn, sd_, nd_ = cut(s), cut(n), cut(s_dry), cut(n_dry)
@@ -213,15 +237,20 @@ def tango_scores(y, s, n, s_dry, n_dry, times, fs, *, stoi=False):
                                                     rows.reshape(B, K * 3, -1).contiguous())
     d_sdr, d_sir, d_sar = (x.view(B, K, 3) for x in (d_sdr, d_sir, d_sar))
 
-    _, snr_out, _ = fw_snr(sf, nf, fs)
-    _, snr_in, _ = fw_snr(ss, nn, fs)
-    _, snr_in_dry, _ = fw_snr(sd_, nd_, fs)
-    _, snr_out_z, _ = fw_snr(szf, nzf, fs)
+    # band statistics: without lengths over the non-zero filter outputs; with lengths over the samples that are both
+    # before the utterance's end and non-zero outputs of the trimmed signal (the outputs are zero exactly up to the
+    # first non-zero input sample: the band-passes have b0 != 0)
+    own = (lambda x: None) if keep is None else (lambda x: _scored_samples(x, keep))
+    sd_k = sd_.unsqueeze(1).expand(B, K, -1)
+    _, snr_out, _ = fw_snr(sf, nf, fs, vad_tar=own(sf), vad_noi=own(nf))
+    _, snr_in, _ = fw_snr(ss, nn, fs, vad_tar=own(ss), vad_noi=own(nn))
+    _, snr_in_dry, _ = fw_snr(sd_, nd_, fs, vad_tar=own(sd_), vad_noi=own(nd_))
+    _, snr_out_z, _ = fw_snr(szf, nzf, fs, vad_tar=own(szf), vad_noi=own(nzf))
     snr_in_dry = snr_in_dry.unsqueeze(1).expand(B, K)
-    _, sd_cnv, _ = fw_sd(sf, ss, fs)
-    _, sd_dry, _ = fw_sd(sf, sd_.unsqueeze(1).expand(B, K, -1), fs)
-    _, sd_cnv_z, _ = fw_sd(szf, ss, fs)
-    _, sd_dry_z, _ = fw_sd(szf, sd_.unsqueeze(1).expand(B, K, -1), fs)
+    _, sd_cnv, _ = fw_sd(sf, ss, fs, sel_out=own(sf), sel_in=own(ss))
+    _, sd_dry, _ = fw_sd(sf, sd_k, fs, sel_out=own(sf), sel_in=own(sd_k))
+    _, sd_cnv_z, _ = fw_sd(szf, ss, fs, sel_out=own(szf), sel_in=own(ss))
+    _, sd_dry_z, _ = fw_sd(szf, sd_k, fs, sel_out=own(szf), sel_in=own(sd_k))
 
     shared = {"snr_in_cnv": snr_in, "snr_in_dry": snr_in_dry,
               "sdr_in_cnv": sdr[..., 2], "sir_in_cnv": sir[..., 2],
@@ -233,15 +262,25 @@ def tango_scores(y, s, n, s_dry, n_dry, times, fs, *, stoi=False):
                 "snr_out": snr_out_z, "fw_sd_cnv": sd_cnv_z, "fw_sd_dry": sd_dry_z,
                 "sar_dry": d_sar[..., 1], "sir_dry": d_sir[..., 1], "sdr_dry": d_sdr[..., 1], **shared}
     if stoi:
-        d = _tango_stoi(ss, sd_, yy, sh, szh, fs)                                # [B, K, 6]
+        d = _tango_stoi(ss, sd_, yy, sh, szh, fs, None if keep is None else lb)  # [B, K, 6]
         results["delta_stoi_cnv"], results["delta_stoi_dry"] = d[..., 1] - d[..., 0], d[..., 4] - d[..., 3]
         resultsz["delta_stoi"], resultsz["delta_stoi_dry"] = d[..., 2] - d[..., 0], d[..., 5] - d[..., 3]
     return results, resultsz
 
 
-def _tango_stoi(s, s_dry, y, sh, szh, fs):
+def _scored_samples(x, keep):
+    """float32 0/1 like x [B, ..., Ls]: samples n with first_b <= n and keep[b, n], first_b the first non-zero sample
+    of the row (Ls for an all-zero row, which then selects nothing)."""
+    nz = x != 0
+    first = torch.where(nz.any(-1), nz.to(torch.int8).argmax(-1), x.shape[-1])
+    n = torch.arange(x.shape[-1], device=x.device)
+    k = keep.view((keep.shape[0],) + (1,) * (x.dim() - 2) + (keep.shape[1],))
+    return ((n >= first.unsqueeze(-1)) & k).to(torch.float32)
+
+
+def _tango_stoi(s, s_dry, y, sh, szh, fs, lengths=None):
     """STOI of the six pairs of every node, [B, K, 6]: (s, y), (s, sh), (s, szh), (s_dry, y), (s_dry, sh),
-    (s_dry, szh).  s, y, sh, szh [B, K, L]; s_dry [B, L]."""
+    (s_dry, szh).  s, y, sh, szh [B, K, L]; s_dry [B, L]; lengths [B] (host, or None): samples per utterance."""
     from . import stoi as _stoi
     B, K, L = s.shape
     cleans = torch.cat((s.reshape(B * K, L), s_dry.reshape(B, L)))               # node cleans, then dry cleans
@@ -251,5 +290,6 @@ def _tango_stoi(s, s_dry, y, sh, szh, fs):
     deg = 3 * node[:, None] + torch.arange(3, device=s.device)                   # [B K, 3]
     cl = torch.stack((node, dry), dim=1)[:, :, None].expand(B * K, 2, 3)         # [B K, 2, 3]
     pairs = torch.stack((cl, deg[:, None, :].expand(B * K, 2, 3)), dim=-1)       # [B K, 2, 3, 2]
-    d = _stoi.stoi_pairs(cleans.contiguous(), degraded.contiguous(), pairs.reshape(-1, 2), fs)
+    lc = None if lengths is None else np.concatenate((np.repeat(lengths, K), lengths))
+    d = _stoi.stoi_pairs(cleans.contiguous(), degraded.contiguous(), pairs.reshape(-1, 2), fs, lengths=lc)
     return d.view(B, K, 6)

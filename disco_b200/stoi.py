@@ -57,14 +57,23 @@ def band_edges():
     return [(int(np.argmin(np.square(f - a))), int(np.argmin(np.square(f - b)))) for a, b in zip(lo, hi)]
 
 
-def to_10k(x, fs):
-    """x [..., L] float32 CUDA tensor at fs -> float64 at 10 kHz (pystoi's resample_oct)."""
+def to_10k(x, fs, lengths=None):
+    """x [..., L] float32 CUDA tensor at fs -> float64 at 10 kHz (pystoi's resample_oct).  lengths (per row, or None):
+    each row is resampled as its first lengths[s] samples, zero after ceil(lengths[s] 10000 / fs)."""
     if int(fs) != fs or fs < 1:
         raise ValueError("fs must be a positive integer rate, got %r" % (fs,))
     if int(fs) == FS:
         return x.double()
     taps, up, down = resample_taps(int(fs))
-    return ops.resample_poly(x, torch.from_numpy(taps).to(x.device), up, down)
+    return ops.resample_poly(x, torch.from_numpy(taps).to(x.device), up, down, lengths=lengths)
+
+
+def length_10k(n, fs):
+    """Samples at 10 kHz of n samples at fs: ceil(n up / down), resample_poly's output length."""
+    if int(fs) == FS:
+        return np.asarray(n)
+    _, up, down = resample_taps(int(fs))
+    return -(-np.asarray(n, dtype=np.int64) * up // down)
 
 
 def _check(t, name):
@@ -80,20 +89,39 @@ def _warn_if_short(n_frames):
                       "frames. Returning 1e-5. Please check you wav files", RuntimeWarning, stacklevel=3)
 
 
-def stoi_pairs(cleans, degraded, pairs, fs):
+def stoi_pairs(cleans, degraded, pairs, fs, lengths=None):
     """STOI of (clean, degraded) pairs.  cleans [C, L], degraded [D, L] float32 CUDA tensors at rate fs, pairs [P, 2]
     integer (clean index, degraded index) -> d [P] float64.  Every signal is resampled once, and every clean's
-    selection and band envelopes are computed once however many pairs share it."""
+    selection and band envelopes are computed once however many pairs share it.
+    lengths [C] (integers, or None): clean c and every degraded signal paired with it are their first lengths[c]
+    samples; a pair scores as pystoi on the two trimmed signals.  A degraded signal paired with cleans of different
+    lengths raises ValueError."""
     _check(cleans, "cleans")
     _check(degraded, "degraded")
     if cleans.dim() != 2 or degraded.dim() != 2 or cleans.shape[1] != degraded.shape[1]:
         raise ValueError("cleans [C, L] / degraded [D, L] shape mismatch: %s / %s"
                          % (tuple(cleans.shape), tuple(degraded.shape)))
     pairs = torch.as_tensor(pairs).to(device=cleans.device, dtype=torch.int32).reshape(-1, 2).contiguous()
-    xc, xd = to_10k(cleans.contiguous(), fs), to_10k(degraded.contiguous(), fs)
+    if lengths is None:
+        xc, xd = to_10k(cleans.contiguous(), fs), to_10k(degraded.contiguous(), fs)
+        l10 = None
+    else:
+        C, D, L = cleans.shape[0], degraded.shape[0], cleans.shape[1]
+        lc = ops.signal_lengths(lengths, (C,), L)
+        pr = pairs.cpu().numpy().astype(np.int64)
+        if pr.size and (pr[:, 0].min() < 0 or pr[:, 0].max() >= C or pr[:, 1].min() < 0 or pr[:, 1].max() >= D):
+            raise IndexError("stoi: pair indices out of range (%d cleans, %d degraded signals)" % (C, D))
+        ld = np.full(D, L, dtype=np.int32)
+        ld[pr[:, 1]] = lc[pr[:, 0]]
+        if np.any(ld[pr[:, 1]] != lc[pr[:, 0]]):
+            raise ValueError("stoi: a degraded signal is paired with cleans of different lengths")
+        xc, xd = to_10k(cleans.contiguous(), fs, lc), to_10k(degraded.contiguous(), fs, ld)
+        l10 = length_10k(lc, fs)
+        if int(l10.min()) < N_FRAME:
+            raise ValueError("stoi: %d samples at 10 kHz; at least %d are needed" % (int(l10.min()), N_FRAME))
     if xc.shape[-1] < N_FRAME:
         raise ValueError("stoi: %d samples at 10 kHz; at least %d are needed" % (xc.shape[-1], N_FRAME))
-    d, _, n_frames = ops.stoi(xc, xd, pairs)
+    d, _, n_frames = ops.stoi(xc, xd, pairs, lengths=l10)
     _warn_if_short(n_frames)
     return d
 

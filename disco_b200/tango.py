@@ -34,16 +34,42 @@ def _bcast_mask(X, m, one_minus):
     return ops.apply_mask(X, m, one_minus)
 
 
-def _ivad_mask(s_ref, n_fft):
+def _ivad_mask(s_ref, n_fft, lengths=None):
     """'ivad' masks (tango.py:216-221): the per-sample energy VAD of the clean reference channel,
-    taken every hop and spread over all bins.  s_ref [B, K, L] -> [B, K, T, F] float32 (0/1); all (b, k) at once."""
+    taken every hop and spread over all bins.  s_ref [B, K, L] -> [B, K, T, F] float32 (0/1); all (b, k) at once.
+    lengths [B] (host, or None): utterance b is its first lengths[b] samples, so its VAD (quantile and framing) is
+    taken over those alone, once per distinct length, and its frames from 1 + lengths[b] // hop on are 0."""
     from .compat.sigproc_utils import vad_oracle_rows_device
     B, K, L = s_ref.shape
     hop, F, T = n_fft // 2, n_fft // 2 + 1, ops.n_frames(L, n_fft)
-    vad = vad_oracle_rows_device(s_ref.reshape(B * K, L), win_len=n_fft, win_hop=hop)[:, ::hop]      # [B*K, <= T]
     out = torch.zeros((B, K, T, F), dtype=torch.float32, device=s_ref.device)
-    out[:, :, :vad.shape[1], :] = vad.to(torch.float32).view(B, K, -1, 1)
+    if lengths is None:
+        vad = vad_oracle_rows_device(s_ref.reshape(B * K, L), win_len=n_fft, win_hop=hop)[:, ::hop]  # [B*K, <= T]
+        out[:, :, :vad.shape[1], :] = vad.to(torch.float32).view(B, K, -1, 1)
+        return out
+    for Lb in sorted({int(v) for v in lengths}):
+        idx = torch.from_numpy(np.flatnonzero(np.asarray(lengths) == Lb)).to(s_ref.device)
+        rows = s_ref.index_select(0, idx)[..., :Lb]
+        vad = vad_oracle_rows_device(rows.reshape(-1, Lb), win_len=n_fft, win_hop=hop)[:, ::hop]
+        out[idx, :, :vad.shape[1], :] = vad.to(torch.float32).view(len(idx), K, -1, 1)
     return out
+
+
+def _uneven_lengths(lengths, B, L, n_fft):
+    """Host int32 [B] lengths of a batch whose utterances do not all have L samples; None for lengths=None or all L
+    (the uniform batch)."""
+    if lengths is None:
+        return None
+    host = ops.signal_lengths(lengths, (B,), L, lo=n_fft // 2)
+    return None if bool((host == L).all()) else host
+
+
+def _frame_clip(lengths, T, n_fft, device):
+    """m -> m with every frame t >= 1 + lengths[b] // hop of utterance b set to 0, for [B, K, T, F] masks (a selection,
+    so that a 0/0 = NaN of an oracle mask on the zero frames past the end is replaced, not multiplied)."""
+    Tb = torch.from_numpy(1 + np.asarray(lengths, dtype=np.int64) // (n_fft // 2)).to(device)
+    past = (torch.arange(T, device=device)[None, :] >= Tb[:, None]).view(-1, 1, T, 1)
+    return lambda m: m.masked_fill(past, 0.0)
 
 
 # network masks see windows of 21 frames, hop 1, and predict the middle one (reference tango.py:34-35, 340)
@@ -86,21 +112,22 @@ def _dnn_masks(mod, Y0, z=None, nodes=None, z_sigs="zs_hat"):
     return torch.stack(out).view(B, n, T, F)
 
 
-def _step1_mask(vad, mods, ref_spectra, s_ref, y_ref, n_fft):
+def _step1_mask(vad, mods, ref_spectra, s_ref, y_ref, n_fft, lengths=None):
     """Step-1 mask [B, K, T, F] of the reference microphone (tango.py:338-342): an oracle type of its clean
     spectra ref_spectra() -> (S_ref, N_ref), 'ivad' of its clean signal s_ref [B, K, L], or mods[0] on its mixture
     spectrum y_ref() [B, K, T, F].  The spectra are callables so that each caller keeps its own STFT grouping
-    (the two-for-one FFT makes a channel's bits depend on its partner signal) and computes only what `vad` needs."""
+    (the two-for-one FFT makes a channel's bits depend on its partner signal) and computes only what `vad` needs.
+    lengths: per-utterance lengths of an uneven batch (for 'ivad'), or None."""
     kind = _mask_kind(vad)
     if kind == "ivad":                                                  # tango.py:216-221
-        return _ivad_mask(s_ref, n_fft)
+        return _ivad_mask(s_ref, n_fft, lengths)
     if kind == "dnn":
         return _dnn_masks(mods[0], y_ref())
     return ops.tf_mask(*ref_spectra(), vad)
 
 
 def _step2_mask(vads, mods, mask_z, ch0_spectra, s0, n_fft, Y0=None, z=None, nodes=None, z_sigs="zs_hat",
-                ref_mic=0):
+                ref_mic=0, lengths=None):
     """Step-2 mask [B, n, T, F] (tango.py:387-394).  mask_z itself for the step-1 oracle kind on the same
     microphone, or for a network step without a model of its own (mods[1] None, tango.py:388-389); otherwise an
     oracle type or 'ivad' of microphone 0 (ch0_spectra, s0 as in _step1_mask) or mods[1] on Y0 [B, n, T, F]
@@ -109,20 +136,23 @@ def _step2_mask(vads, mods, mask_z, ch0_spectra, s0, n_fft, Y0=None, z=None, nod
         return mask_z if mods[1] is None else _dnn_masks(mods[1], Y0, z, nodes, z_sigs)
     if vads[1] == vads[0] and ref_mic == 0:
         return mask_z
-    return _step1_mask(vads[1], None, ch0_spectra, s0, None, n_fft)
+    return _step1_mask(vads[1], None, ch0_spectra, s0, None, n_fft, lengths)
 
 
-def _z_for_stats(mask_for_z, vads, Z, mask_w, Zs, Zn, oracle_refs):
+def _z_for_stats(mask_for_z, vads, Z, mask_w, Zs, Zn, oracle_refs, clip=None):
     """What the other nodes contribute to the step-2 speech / noise statistics (tango.py:396-429): (z_rs, z_rn)
     [B, K, T, F] from the compressed signals Z, the step-2 masks mask_w, the filtered clean components Zs, Zn and
     oracle_refs() -> clean spectra of the reference microphones; (None, None) for 'local', where z is masked by
-    the step-2 mask of the node being filtered."""
+    the step-2 mask of the node being filtered.  clip: zeroes the frames past each utterance's end of a mask
+    (uneven batches), or None."""
     if mask_for_z == "local":
         return None, None
     if mask_for_z == "distant":
         return ops.apply_mask(Z, mask_w, False), ops.apply_mask(Z, mask_w, True)
     if mask_for_z == "compressed":
         mc = ops.tf_mask(Zs, Zn, vads[0])
+        if clip is not None:
+            mc = clip(mc)
         return ops.apply_mask(Z, mc, False), ops.apply_mask(Z, mc, True)
     if mask_for_z == "use_oracle_refs":
         return oracle_refs()
@@ -150,14 +180,17 @@ def _reference_lists(res, names, vads, masks=None):
 
 
 def tango_step1(y, mask_z, n_fft=512, mu=1.0, filter_type="gevd", rank=1, ref_mic=0, oracle_sn=None,
-                apply_filter=True):
+                apply_filter=True, lengths=None):
     """y [B, K, C, L] float32, mask_z [B, K, T, F] float32 (frame-major).
     Returns dict: Y [B,K,C,T,F], z_y, zn [B,K,T,F], W1 [B,K,F,C], R_ss, R_nn.
     oracle_sn = (S, N) spectra replaces the masked estimates in the SCMs ('use_oracle_*', tango.py:343-345).
-    apply_filter=False leaves z_y / zn to a fused later pass (single-node arrays)."""
+    apply_filter=False leaves z_y / zn to a fused later pass (single-node arrays).
+    lengths [B] (host ints, or None): utterances of their own lengths; Y is then stft_lengths' (zero past each
+    utterance's frames) and the matrices are the sums over its frames divided by T = 1 + L // hop, not by its own
+    frame count (a common scale of R_ss and R_nn, which the filters do not depend on)."""
     B, K, C, L = y.shape
     T, F = ops.n_frames(L, n_fft), n_fft // 2 + 1
-    fused = oracle_sn is None and ops.stft_scm_supported(n_fft, C, 1)
+    fused = oracle_sn is None and lengths is None and ops.stft_scm_supported(n_fft, C, 1)
     if fused and C <= 4:
         # fused STFT + SCM; the solve reads the per-segment partial sums directly (no finalize launch)
         Y, ws = ops.stft_scm(y.view(B * K, C, L), mask_z.view(B * K, T, F), n_fft, keep_partials=True)
@@ -173,7 +206,7 @@ def tango_step1(y, mask_z, n_fft=512, mu=1.0, filter_type="gevd", rank=1, ref_mi
         Y, Rss, Rnn = ops.stft_scm(y.view(B * K, C, L), mask_z.view(B * K, T, F), n_fft)
         Y, Rss, Rnn = Y.view(B, K, C, T, F), Rss.view(B, K, F, C, C), Rnn.view(B, K, F, C, C)
     else:
-        Y = ops.stft(y, n_fft)
+        Y = ops.stft(y, n_fft) if lengths is None else ops.stft_lengths(y, lengths, n_fft)
         if oracle_sn is None:
             Rss, Rnn = ops.masked_scm(Y, mask_z, None, n_fft)
         else:
@@ -205,7 +238,7 @@ def tango_step2(Y, Z, mask_w, n_fft=512, mu=1.0, filter_type="gevd", rank=1, out
 
 
 def tango_batched(y, s=None, n=None, masks=None, vads=("irm1", "irm1"), mask_for_z="local", n_fft=512,
-                  mu=1.0, filter_type="gevd", rank=1, ref_mic=0, out_layout="FT", diagnostics=True):
+                  mu=1.0, filter_type="gevd", rank=1, ref_mic=0, out_layout="FT", diagnostics=True, lengths=None):
     """Batched two-step Tango.
 
     y [B, K, C, L] float32 CUDA tensor (K nodes of C microphones).  Masks come either from the
@@ -216,10 +249,20 @@ def tango_batched(y, s=None, n=None, masks=None, vads=("irm1", "irm1"), mask_for
     Returns a dict with the reference's outputs (tango.py:457) as [B, K, F, T] (out_layout='FT') or
     [B, K, T, F] ('TF') tensors: yf, z_y, zn, masks_z, mask_w and, with s/n and diagnostics, sf, nf,
     z_s, z_n.
+
+    lengths: one length per utterance ([B] integers, n_fft/2 < lengths[b] <= L), or None.  Utterance b is then its
+    first lengths[b] samples (y, s, n zero after them) and has T_b = 1 + lengths[b] // hop frames: its outputs are
+    those of the utterance alone, trimmed, to rounding, and every output (masks included) is exactly 0 from frame
+    T_b on.  Such a batch runs the routes that store the spectra (the fused STFT+SCM kernels assume one length);
+    lengths=None or all lengths equal to L is the uniform batch, computed exactly as without the argument.
     """
     if mask_for_z is None:
         raise TypeError("argument of type 'NoneType' is not iterable")   # reference tango.py:343
     B, K, C, L = y.shape
+    T, F = ops.n_frames(L, n_fft), n_fft // 2 + 1
+    lens = _uneven_lengths(lengths, B, L, n_fft)
+    stft = (lambda a: ops.stft(a, n_fft)) if lens is None else (lambda a: ops.stft_lengths(a, lens, n_fft))
+    clip = None if lens is None else _frame_clip(lens, T, n_fft, y.device)
     oracle = masks is None
     if oracle and (s is None or n is None):
         raise ValueError("either masks or the clean components (s, n) are required")
@@ -228,29 +271,34 @@ def tango_batched(y, s=None, n=None, masks=None, vads=("irm1", "irm1"), mask_for
         raise ValueError("mask_for_z=%r needs the clean components s and n" % mask_for_z)
     S = N = None
     if have_sn and (oracle or diagnostics or "use_oracle_" in mask_for_z):
-        S, N = ops.stft(s, n_fft), ops.stft(n, n_fft)
+        S, N = stft(s), stft(n)
     # ---- masks
     if oracle:
         if "dnn" in [_mask_kind(v) for v in vads]:
             raise ValueError("network masks ('crnn' / 'rnn') come in through masks=")
         spectra = lambda ch: (_ref_plane(S, ch), _ref_plane(N, ch))
-        mask_z = _step1_mask(vads[0], None, lambda: spectra(ref_mic), s[:, :, ref_mic], None, n_fft)
-        mask_w = _step2_mask(vads, None, mask_z, lambda: spectra(0), s[:, :, 0], n_fft, ref_mic=ref_mic)
+        mask_z = _step1_mask(vads[0], None, lambda: spectra(ref_mic), s[:, :, ref_mic], None, n_fft, lens)
+        mask_w = _step2_mask(vads, None, mask_z, lambda: spectra(0), s[:, :, 0], n_fft, ref_mic=ref_mic,
+                             lengths=lens)
     else:
         mask_z, mask_w = masks
         if mask_w is None:
             mask_w = mask_z
+    if clip is not None:
+        # past an utterance's end its spectra are 0 and an oracle mask 0/0: every mask is 0 there
+        mz = clip(mask_z)
+        mask_w = mz if mask_w is mask_z else (mask_w if callable(mask_w) else clip(mask_w))
+        mask_z = mz
     # mask_w may be a callable (Y, z_y, zn) -> [B, K, T, F]: a step-2 mask estimator that looks at the
     # compressed signals of the other nodes (tango.py:387-394)
     mask_w_fn = mask_w if callable(mask_w) else None
     # ---- step 1
     osn = (S, N) if "use_oracle_" in mask_for_z else None
-    T, F = ops.n_frames(L, n_fft), n_fft // 2 + 1
     # single-node arrays with both masks known: the step-2 statistics are taken over the same Y as the step-1
     # statistics (tango.py:431-440 with K = 1), so ONE pass accumulates both and ONE pass applies both filters
     single = (K == 1 and mask_for_z == "local" and mask_w_fn is None and osn is None)
     same_mask = single and mask_w is mask_z
-    fuse_dual = single and not same_mask and ops.stft_scm_supported(n_fft, C, 2)
+    fuse_dual = single and not same_mask and lens is None and ops.stft_scm_supported(n_fft, C, 2)
     # otherwise for single-node arrays: the step-1 filter-and-sum and the step-2 SCM share one pass over Y
     fuse_mid = (single and not same_mask and not fuse_dual and C <= 8)
     # multi-node arrays: z of every node + the step-2 SCMs of every node in one pass over Y
@@ -270,10 +318,12 @@ def tango_batched(y, s=None, n=None, masks=None, vads=("irm1", "irm1"), mask_for
         final_layout = True
     else:
         st1 = tango_step1(y, mask_z, n_fft, mu, filter_type, rank, ref_mic, oracle_sn=osn,
-                          apply_filter=not (fuse_mid or fuse_multi))
+                          apply_filter=not (fuse_mid or fuse_multi), lengths=lens)
         Y, z_y, zn, W1 = st1["Y"], st1["z_y"], st1["zn"], st1["W1"]
         if mask_w_fn is not None:
             mask_w = mask_w_fn(Y, z_y, zn)
+            if clip is not None:
+                mask_w = clip(mask_w)
         if same_mask:
             # K = 1 and mask_w is mask_z (tango.py:388-389): the step-2 statistics ARE the step-1 statistics,
             # so w_glo = w_loc and yf = z
@@ -289,7 +339,7 @@ def tango_batched(y, s=None, n=None, masks=None, vads=("irm1", "irm1"), mask_for
         z_s = ops.filter_sum(W1, S, None, conj=True, n_fft=n_fft)
         z_n = ops.filter_sum(W1, N, None, conj=True, n_fft=n_fft)
     z_rs, z_rn = _z_for_stats(mask_for_z, vads, z_y, mask_w, z_s, z_n,
-                              lambda: (_ref_plane(S, ref_mic), _ref_plane(N, ref_mic)))
+                              lambda: (_ref_plane(S, ref_mic), _ref_plane(N, ref_mic)), clip)
     # ---- step 2
     ft = ops._layout(out_layout) == ops.FT
     conv = ops.transpose_last2 if ft else (lambda a: a)

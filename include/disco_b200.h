@@ -220,6 +220,24 @@ DISCO_API int disco_filter_dual(const void* W1, const void* W2, const void* Y, v
  *   Y [n_sig][T][F] complex64 (frame-major) -> x [n_sig][length] float32 */
 DISCO_API int disco_istft(const void* Y, float* x, int n_sig, int T, int length, int n_fft, void* stream);
 
+/* ---- STFT / iSTFT of signals of different lengths ---------------------------------------------------
+ * A batch of n_sig signals held in rows of `length` samples, signal s being lengths[s] samples long and zero after
+ * that (n_fft/2 < lengths[s] <= length).  It has T_s = 1 + lengths[s] / hop frames.
+ * disco_stft_lengths: x [n_sig][length] -> Y [n_sig][T][F], T = 1 + length / hop.  Frame t < T_s is disco_stft's
+ *   frame of the signal trimmed to lengths[s] (reflect padding at ITS end); frames T_s .. T - 1 are 0.  Signals 2p and
+ *   2p + 1 share one complex transform as in disco_stft, so a frame is bit-identical to disco_stft of the trimmed
+ *   pair when both signals of the pair have the same length.
+ * disco_istft_lengths: Y [n_sig][T][F] -> x [n_sig][length].  Samples < lengths[s] are disco_istft of frames
+ *   [0, min(T, T_s)) of signal s to lengths[s] samples (bit-identical when both signals of the pair have the same
+ *   length; a pair of different lengths runs each signal alone, as disco_istft runs a single signal); samples from
+ *   lengths[s] on are 0.
+ * `lengths` is the device copy of the lengths the kernels read; `lengths_host` holds the same values in host memory
+ * and is checked before anything is launched (DISCO_ERR_INVALID for a length out of range or a NULL pointer). */
+DISCO_API int disco_stft_lengths(const float* x, const int* lengths, const int* lengths_host, void* Y, int n_sig,
+                                 int length, int n_fft, void* stream);
+DISCO_API int disco_istft_lengths(const void* Y, const int* lengths, const int* lengths_host, float* x, int n_sig,
+                                  int T, int length, int n_fft, void* stream);
+
 /* ---- recursive (online) statistics and block-wise filtering ------------------------------------------
  * disco_scm_recursive evaluates, for every frame t and bin, the reference's one-frame update
  *   spatial_correlation_matrix(Rxx, x, lambda_cor, M):  R <- lambda R + (1 - lambda) [M] x x^H
@@ -318,6 +336,20 @@ DISCO_API size_t disco_stoi_workspace(int n_clean, int n_pair, int length);
 DISCO_API int disco_stoi(const double* cleans, const double* degraded, const int* pairs, double* d, int* n_sel,
                          int* n_frames, int n_clean, int n_deg, int n_pair, int length, void* workspace,
                          size_t workspace_bytes, void* stream);
+/* The same for signals of their own lengths in rows of `length` samples (the rows are zero after them):
+ *   disco_resample_poly_lengths: row s is its first lengths[s] samples (1 <= lengths[s] <= length); output samples
+ *     < ceil(lengths[s] up / down) are disco_resample_poly's of the trimmed row, the rest of the output row is 0.
+ *   disco_stoi_lengths: clean c, and every degraded signal paired with it, is its first lengths[c] samples
+ *     (256 <= lengths[c] <= length): the frame selection stops at the last full frame of those, so a pair scores as
+ *     disco_stoi on the trimmed signals does.  With lengths[c] = length for every clean it equals disco_stoi.
+ * `lengths` is the device copy the kernels read; `lengths_host` the same values in host memory, checked first
+ * (DISCO_ERR_INVALID for a length out of range or a NULL pointer). */
+DISCO_API int disco_resample_poly_lengths(const float* x, double* y, const double* taps, int n_taps, int up, int down,
+                                          int n_sig, int length, const int* lengths, const int* lengths_host,
+                                          void* stream);
+DISCO_API int disco_stoi_lengths(const double* cleans, const double* degraded, const int* pairs, double* d, int* n_sel,
+                                 int* n_frames, int n_clean, int n_deg, int n_pair, int length, const int* lengths,
+                                 const int* lengths_host, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- layout helpers -------------------------------------------------------------------------------
  * out[b][c][r] = in[b][r][c] for `batch` planes (complex64 / float32).  Used at the Python

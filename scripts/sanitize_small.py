@@ -55,3 +55,27 @@ with warnings.catch_warnings():
     d_short = stoi.stoi(x[:, :3000], x[:, :3000], 16000)
 torch.cuda.synchronize()
 print("ok stoi", d.tolist(), d_short.tolist())
+# signals of their own lengths: length-aware STFT / iSTFT at every n_fft (odd signal counts, pairs of equal and of
+# different lengths, a signal of hop + 1 samples), the length-aware resampler and STOI selection, an uneven Tango batch
+for n_fft in (256, 512, 1024):
+    H = n_fft // 2
+    L = 9 * H + 37
+    lengths = [L, H + 1, L - H - 3, L - H - 3, 5 * H + 1]
+    x = torch.randn(len(lengths), L, device=dev)
+    for i, Lb in enumerate(lengths):
+        x[i, Lb:] = 0
+    Y = ops.stft_lengths(x, lengths, n_fft)
+    xr = ops.istft_lengths(Y, lengths, L, n_fft)
+    torch.cuda.synchronize()
+    print("ok lengths", n_fft, float((xr - x).abs().max()))
+with warnings.catch_warnings():
+    warnings.simplefilter("ignore", RuntimeWarning)
+    x = torch.randn(3, 24000, device=dev) * (torch.arange(24000, device=dev) % 8000 < 5000)
+    d = stoi.stoi_pairs(x, x + 0.3 * torch.randn_like(x), [(0, 0), (1, 1), (2, 2)], 16000, lengths=[24000, 9001, 17777])
+torch.cuda.synchronize()
+y, s, n = make_batch(3, 2, 2, 9000, seed0=2)
+out = tango_batched(torch.from_numpy(y).to(dev), torch.from_numpy(s).to(dev), torch.from_numpy(n).to(dev),
+                    lengths=[9000, 5001, 7003])
+td = post.to_time(out, 9000, lengths=[9000, 5001, 7003])
+torch.cuda.synchronize()
+print("ok lengths stoi / tango", d.tolist(), float(td["yf"].abs().mean()))
