@@ -15,7 +15,7 @@ ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(ROOT, "build", "obj")
 LIB = os.path.join(HERE, "libdisco_b200.so")
-SOURCES = ["api.cu", "stft_scm.cu", "scm.cu", "scm_wide.cu", "solve.cu", "solve_small.cu", "filter_sum.cu", "filter_sum_multi.cu", "filter_dual.cu", "mid_multi.cu", "istft.cu", "filterbank.cu", "online.cu", "misc.cu", "stream.cu", "bss.cu", "stoi.cu", "lengths.cu"]
+SOURCES = ["api.cu", "stft_scm.cu", "scm.cu", "scm_wide.cu", "solve.cu", "solve_small.cu", "filter_sum.cu", "filter_sum_multi.cu", "filter_dual.cu", "mid_multi.cu", "istft.cu", "filterbank.cu", "online.cu", "online_wide.cu", "misc.cu", "stream.cu", "bss.cu", "stoi.cu", "lengths.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
          "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden"]

@@ -571,7 +571,6 @@ int disco_scm_recursive(const void* Y, const void* Z, const float* mask, const v
     memset(&a, 0, sizeof(a));
     int rc = make_cat(&a.in, Y, Z, n_utt, K, C, T, n_fft, node_sel, n_sel);
     if (rc) return rc;
-    if (C + K - 1 > 8) return fail(DISCO_ERR_UNSUPPORTED, "recursive SCM: C + K - 1 must be <= 8");
     if (a.in.n_grp > kMaxGridYZ) return fail(DISCO_ERR_UNSUPPORTED, "at most 65535 (utterance, node) groups per call");
     if (!Rss || !Rnn || (!R0ss) != (!R0nn)) return fail(DISCO_ERR_INVALID, "null pointer");
     if (block < 1 || block > 64) return fail(DISCO_ERR_INVALID, "block must be 1..64 frames");
@@ -603,7 +602,6 @@ int disco_filter_sum_blocks(const void* W, int conj_w, const void* Y, const void
     memset(&a, 0, sizeof(a));
     int rc = make_cat(&a.in, Y, Z, n_utt, K, C, T, n_fft, node_sel, n_sel);
     if (rc) return rc;
-    if (C + K - 1 > 8) return fail(DISCO_ERR_UNSUPPORTED, "block filter: C + K - 1 must be <= 8");
     if (a.in.n_grp > kMaxGridYZ) return fail(DISCO_ERR_UNSUPPORTED, "at most 65535 (utterance, node) groups per call");
     if (!W || !out) return fail(DISCO_ERR_INVALID, "null pointer");
     if (block < 1 || block > 64 || lag < 0) return fail(DISCO_ERR_INVALID, "bad block / lag");

@@ -194,6 +194,9 @@ struct OnlineArgs {
     float gw[64];           // (1 - lambda) lambda^k, k = 0..P-1
 };
 cudaError_t launch_scm_recursive(const OnlineArgs& a, cudaStream_t st);
+// D = 9..16 (online_wide.cu): a CTA per (group, 32-bin block) streams the frames and carries R_(j-1) itself; same
+// values as launch_scm_recursive's two-level scan.  Reads of R0: upper triangle, real part of the diagonal.
+cudaError_t launch_scm_recursive_wide(const OnlineArgs& a, cudaStream_t st);
 
 struct OnlineFilterArgs {
     CatArgs in;
@@ -204,6 +207,7 @@ struct OnlineFilterArgs {
     int ref, P, J, lag;     // frame t uses filter t / P - lag (pass-through of channel `ref` while that is < 0)
 };
 cudaError_t launch_filter_sum_blocks(const OnlineFilterArgs& a, cudaStream_t st);
+cudaError_t launch_filter_sum_blocks_wide(const OnlineFilterArgs& a, cudaStream_t st);   // D = 9..16
 
 // IIR filter bank + band statistics (filterbank.cu; reference metrics.py fw_snr / fw_sd).
 struct BankArgs {

@@ -139,7 +139,7 @@ cudaError_t launch_scm_recursive(const OnlineArgs& a, cudaStream_t st) {
         case 6: return launch_blocks_d<6>(a, st);
         case 7: return launch_blocks_d<7>(a, st);
         case 8: return launch_blocks_d<8>(a, st);
-        default: return cudaErrorNotSupported;
+        default: return launch_scm_recursive_wide(a, st);   // D = 9..16: online_wide.cu
     }
 }
 
@@ -153,6 +153,21 @@ cudaError_t launch_filter_sum_blocks(const OnlineFilterArgs& a, cudaStream_t st)
         case 6: return launch_filter_d<6>(a, st);
         case 7: return launch_filter_d<7>(a, st);
         case 8: return launch_filter_d<8>(a, st);
+        default: return launch_filter_sum_blocks_wide(a, st);
+    }
+}
+
+// D = 9..16: the same block filter (its registers hold the D taps and one frame's D operands, no pairs)
+cudaError_t launch_filter_sum_blocks_wide(const OnlineFilterArgs& a, cudaStream_t st) {
+    switch (a.in.C + a.in.K - 1) {
+        case 9: return launch_filter_d<9>(a, st);
+        case 10: return launch_filter_d<10>(a, st);
+        case 11: return launch_filter_d<11>(a, st);
+        case 12: return launch_filter_d<12>(a, st);
+        case 13: return launch_filter_d<13>(a, st);
+        case 14: return launch_filter_d<14>(a, st);
+        case 15: return launch_filter_d<15>(a, st);
+        case 16: return launch_filter_d<16>(a, st);
         default: return cudaErrorNotSupported;
     }
 }

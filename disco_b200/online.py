@@ -7,9 +7,13 @@ step: exponentially smoothed masked SCMs, a filter refreshed every `block` frame
 so far, applied to the following frames.  Here that composition is three batched launches over all
 utterances, nodes, bins and blocks (csrc/online.cu + the batched solver):
 
-    scm_recursive      two-level scan of the recursion -> (R_ss, R_nn) after every block
+    scm_recursive      scan of the recursion -> (R_ss, R_nn) after every block; D = C + K - 1 <= 8: two levels
+                       (block sums, then the combine), 9..16: one staged pass that carries R (same values)
     mwf_solve          one GEVD-MWF per (block, bin)
     filter_sum_blocks  frame t filtered with the filter of block t // block - lag
+
+Every channel stack up to D = 16 runs, the MEETIT geometry (8 nodes x 2 mics, step 2 at D = 9) included;
+the chunked `stream.OnlineTangoStream` covers D <= 8.
 
 `lag = 1` is strictly causal with an algorithmic delay of 0 frames (the filter in force was finished before
 the frame arrived); `lag = 0` uses the block's own statistics (look-ahead of up to block - 1 frames).

@@ -496,7 +496,8 @@ def scm_recursive(Y, mask, Z=None, lambda_cor=0.95, block=8, power=2, R0=None, n
     """Exponentially smoothed SCM pair, R <- lambda R + (1 - lambda) w x x^H per frame (reference
     spatial_correlation_matrix, internal_formulas.py:84-103), sampled after every block of `block` frames.
     Y [B, Ksel, C, T, F], Z [B, K, T, F] or None, mask [B, Ksel, T, F] or None, R0 = (R0ss, R0nn) [B, Ksel, F, D, D]
-    -> Rss, Rnn [B, Ksel, J, F, D, D], J = ceil(T / block)."""
+    -> Rss, Rnn [B, Ksel, J, F, D, D], J = ceil(T / block), D = C + K - 1 <= 16.  At D >= 9 only the upper triangle
+    and the real diagonal of R0 are read (R0 is Hermitian); the values are those of the D <= 8 two-level scan."""
     n_utt, K, sel, n_sel, _ = _cat_args(Y, Z, node_sel)
     if mask is not None:
         _need(mask, torch.float32, "mask")
@@ -523,7 +524,7 @@ def scm_recursive(Y, mask, Z=None, lambda_cor=0.95, block=8, power=2, R0=None, n
 @_on_device
 def filter_sum_blocks(W, Y, Z=None, block=8, lag=1, conj=True, ref=0, n_fft=512, node_sel=None):
     """One filter per block of frames: out[t] = W[t // block - lag]^H x[t] (pass-through of channel `ref` while no
-    filter exists yet).  W [B, Ksel, J, F, D] -> out, resid = x[ref] - out, [B, Ksel, T, F]."""
+    filter exists yet).  W [B, Ksel, J, F, D], D = C + K - 1 <= 16 -> out, resid = x[ref] - out, [B, Ksel, T, F]."""
     _need(W, torch.complex64, "W")
     n_utt, K, sel, n_sel, _ = _cat_args(Y, Z, node_sel)
     B, Ks, C, T, F = Y.shape

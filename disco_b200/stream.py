@@ -78,7 +78,8 @@ class OnlineTangoStream:
             raise ValueError("lag must be positive")
         D = C + K - 1
         if D > 8:
-            raise NotImplementedError("the recursive kernels cover C + K - 1 <= 8 channels, got %d" % D)
+            raise NotImplementedError("the stream covers C + K - 1 <= 8 channels, got %d (the whole-signal "
+                                      "online_tango goes to 16)" % D)
         if not 0 <= int(ref_mic) < C:
             raise ValueError("ref_mic must be in 0..C-1")
         if R0 is not None:

@@ -243,10 +243,15 @@ DISCO_API int disco_istft_lengths(const void* Y, const int* lengths, const int* 
  *   spatial_correlation_matrix(Rxx, x, lambda_cor, M):  R <- lambda R + (1 - lambda) [M] x x^H
  * (se_utils/internal_formulas.py:84-103) for the pair (R_ss, R_nn) on the concatenated channel view of
  * disco_masked_scm, as a two-level scan, and returns the matrices after the last frame of every block of
- * `block` frames (1..64):  Rss, Rnn [n_utt*n_sel][J][F][D][D], J = ceil(T / block), D = C + K - 1 <= 8.
+ * `block` frames (1..64):  Rss, Rnn [n_utt*n_sel][J][F][D][D], J = ceil(T / block), D = C + K - 1 <= 16.
+ * Every entry is the same float32 value at every D, batch position and launch geometry: A_j = the sequential sum
+ * over block j's frames in frame order, R_j = fmaf(lambda^(frames of block j), R_(j-1), A_j).  A call on frames
+ * [jP, T) with R0 = the matrices after block j - 1 returns the whole call's blocks j, j + 1, ... bit for bit.
  *   weight_power 2: weights m^2 and (1-m)^2 (the caller would pass x = m y, (1-m) y with M = None);
  *   weight_power 1: weights m and 1-m       (x = mixture, M = mask);   mask NULL: weight 1 into Rss, Rnn decays.
- *   R0ss, R0nn: optional initial matrices [n_utt*n_sel][F][D][D] (NULL = zeros).
+ *   R0ss, R0nn: optional initial matrices [n_utt*n_sel][F][D][D] (NULL = zeros), Hermitian.  At D <= 8 every entry
+ *   is read; at D >= 9 only the upper triangle (r <= c) and of the diagonal only the real part, the rest is taken
+ *   as the conjugate mirror and 0.  (Both agree on an exactly Hermitian R0 with a real diagonal.)
  * disco_filter_sum_blocks applies one filter per block: frame t gets W[.., t / block - lag, ..]
  * (lag = 1: the filter of the last completed block, strictly causal; while that index is negative the
  * reference channel passes through), out = w^H x (conj_w = 1), resid = x[ref] - out (optional). */

@@ -26,8 +26,10 @@ for (B, K, C, T, n_fft) in ((2, 1, 8, 37, 512), (2, 4, 4, 21, 256), (1, 8, 2, 9,
         ops.filter_sum_scm(W, Y, m, ref=1, n_fft=n_fft)
     elif ops.tango_mid_supported(C, K):
         ops.tango_mid(W, Y, m, ref=0, n_fft=n_fft)
-    if C + K - 1 <= 8:
-        o = online.online_mwf(Y, m, Z, block=4, lag=1, n_fft=n_fft)
+    o = online.online_mwf(Y, m, Z, block=4, lag=1, n_fft=n_fft)     # D 9..16: online_wide.cu
+    if C + K - 1 > 8:   # the staged scan with R0, a block straddling its ring and a short last block
+        Rs0 = torch.eye(C + K - 1, dtype=torch.complex64, device=dev).expand(B, K, F, C + K - 1, C + K - 1).contiguous()
+        ops.scm_recursive(Y, m, Z, 0.9, 5, 2, (Rs0, Rs0.clone()), n_fft)
     torch.cuda.synchronize()
     print("ok wide", B, K, C, T, n_fft, float(Rs.abs().mean()))
 # online Tango stream: streaming STFT / iSTFT with carried history, block buffers, a partial last block
