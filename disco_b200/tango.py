@@ -270,7 +270,7 @@ def tango_batched(y, s=None, n=None, masks=None, vads=("irm1", "irm1"), mask_for
     if not have_sn and mask_for_z in ("compressed", "use_oracle_refs", "use_oracle_zs"):
         raise ValueError("mask_for_z=%r needs the clean components s and n" % mask_for_z)
     S = N = None
-    if have_sn and (oracle or diagnostics or "use_oracle_" in mask_for_z):
+    if have_sn and (oracle or diagnostics or "use_oracle_" in mask_for_z or mask_for_z == "compressed"):
         S, N = stft(s), stft(n)
     # ---- masks
     if oracle:

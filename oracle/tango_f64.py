@@ -104,10 +104,15 @@ def stft64(x, n_fft=512, hop=256):
 
 
 def offline_tango(y, s=None, n=None, masks=None, n_fft=512, n_hop=256, mu=1.0,
-                  filter_type="gevd", rank=1, mask_for_z="local", mask_power=1, solve=solve):
+                  filter_type="gevd", rank=1, mask_for_z="local", mask_power=1, solve=solve, ref_mic=0):
     """Two-step Tango in float64.  y (K,C,L).  Either (s, n) for oracle irm masks or
     masks=(mask_z (K,F,T), mask_w (K,F,T)).  `solve(Rss, Rnn, mu, filter_type, rank) -> w` is the per-bin
-    filter (e.g. the solver-policy oracle of oracle/solve_f64.py).  Returns dict of (K,F,T) arrays."""
+    filter (e.g. the solver-policy oracle of oracle/solve_f64.py).  Returns dict of (K,F,T) arrays.
+
+    ref_mic: the reference microphone of every node.  Its oracle mask is the step-1 mask of all the node's
+    channels and zn = Y[ref_mic] - z_y; the step-2 oracle mask is that of microphone 0 (as oracle/tango_np.py
+    states it; the reference itself fails for ref_mic != 0, see DESIGN §2).  The filters still estimate the
+    speech at microphone 0 (intern_filter's e_0 selector)."""
     y = np.asarray(y)
     K, C, _ = y.shape
     Y = np.array([[stft64(c, n_fft, n_hop) for c in y[k]] for k in range(K)])
@@ -116,8 +121,8 @@ def offline_tango(y, s=None, n=None, masks=None, n_fft=512, n_hop=256, mu=1.0,
         S = np.array([[stft64(c, n_fft, n_hop) for c in s[k]] for k in range(K)])
         N = np.array([[stft64(c, n_fft, n_hop) for c in n[k]] for k in range(K)])
     if masks is None:
-        mz = np.array([irm(S[k, 0], N[k, 0], mask_power) for k in range(K)])
-        mw = mz
+        mz = np.array([irm(S[k, ref_mic], N[k, ref_mic], mask_power) for k in range(K)])
+        mw = mz if ref_mic == 0 else np.array([irm(S[k, 0], N[k, 0], mask_power) for k in range(K)])
     else:
         mz, mw = np.asarray(masks[0], np.float64), np.asarray(masks[1], np.float64)
     out = {}
@@ -146,7 +151,7 @@ def offline_tango(y, s=None, n=None, masks=None, n_fft=512, n_hop=256, mu=1.0,
         if have_sn:
             sf[k] = filter_sum(w, np.concatenate([S[k], z_s[others]], axis=0))
             nf[k] = filter_sum(w, np.concatenate([N[k], z_n[others]], axis=0))
-    out.update(yf=yf, z_y=z_y, zn=Y[:, 0] - z_y, masks_z=mz, mask_w=mw, Y=Y)
+    out.update(yf=yf, z_y=z_y, zn=Y[:, ref_mic] - z_y, masks_z=mz, mask_w=mw, Y=Y)
     if have_sn:
         out.update(sf=sf, nf=nf, z_s=z_s, z_n=z_n)
     return out

@@ -138,8 +138,12 @@ def concatenate_signals(y, z, k, m=1):
 def offline_tango(y, s, n, vads=("irm1", "irm1"), mask_for_z="local", n_fft=512, n_hop=256,
                   mu=1, filter_type="gevd", rank=1, ref_mic=0, granularity="frame",
                   masks=None, double=False):
-    """tango.py:252-457 with oracle masks (mods=None) and ref_mics = 0.
+    """tango.py:252-457 with oracle masks (mods=None) and the reference microphone ref_mic of every node.
 
+    ref_mic: the step-1 oracle mask is that of microphone ref_mic and applies to all the node's channels, and
+    zn = Y[ref_mic] - z_y; the step-2 oracle mask is that of microphone 0.  The reference pins only ref_mic = 0
+    (for any other value its tango.py:347 reads mask_z before node 0 has one); oracle/tango_f64.py states the same
+    definition independently and tests/test_tango_routes_cpu.py holds the two together.
     y, s, n: [node][channel] 1-D float32 signals.  ``masks`` optionally overrides the
     oracle masks with externally supplied ones: (mask_z[K], mask_w[K]) of (F, T) arrays
     (what a DNN would deliver, tango.py:209-215).
