@@ -60,6 +60,12 @@ SIGNATURES = {
                                     c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int_p, c_int, c_void_p]),
     "disco_filter_sum_blocks": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
                                         c_int, c_int, c_int, c_int, c_int, c_int_p, c_int, c_void_p]),
+    "disco_scm_recursive_lengths": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                            ctypes.c_double, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int_p,
+                                            c_int, c_void_p, c_int_p, c_void_p]),
+    "disco_filter_sum_blocks_lengths": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
+                                                c_int, c_int, c_int, c_int, c_int, c_int, c_int_p, c_int, c_void_p,
+                                                c_int_p, c_void_p]),
     "disco_stream_stft": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                   c_int, c_int, c_int, c_int, c_void_p]),
     "disco_stream_istft": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int,

@@ -564,10 +564,12 @@ int disco_istft_lengths(const void* Y, const int* lengths, const int* lengths_ho
     return 0;
 }
 
-int disco_scm_recursive(const void* Y, const void* Z, const float* mask, const void* R0ss, const void* R0nn, void* Rss,
-                        void* Rnn, double lambda_cor, int block, int weight_power, int n_utt, int K, int C, int T,
-                        int n_fft, const int* node_sel, int n_sel, void* stream) {
-    OnlineArgs a;
+// disco_scm_recursive and, with frames / frames_host, disco_scm_recursive_lengths
+static int scm_recursive_common(const void* Y, const void* Z, const float* mask, const void* R0ss, const void* R0nn,
+                                void* Rss, void* Rnn, double lambda_cor, int block, int weight_power, int n_utt, int K,
+                                int C, int T, int n_fft, const int* node_sel, int n_sel, const int* frames,
+                                const int* frames_host, void* stream) {
+    OnlineLengthsArgs a;
     memset(&a, 0, sizeof(a));
     int rc = make_cat(&a.in, Y, Z, n_utt, K, C, T, n_fft, node_sel, n_sel);
     if (rc) return rc;
@@ -576,6 +578,11 @@ int disco_scm_recursive(const void* Y, const void* Z, const float* mask, const v
     if (block < 1 || block > 64) return fail(DISCO_ERR_INVALID, "block must be 1..64 frames");
     if (!(lambda_cor >= 0.0 && lambda_cor < 1.0)) return fail(DISCO_ERR_INVALID, "lambda_cor must be in [0, 1)");
     if (weight_power != 1 && weight_power != 2) return fail(DISCO_ERR_INVALID, "weight_power must be 1 or 2");
+    if (frames_host) {
+        rc = check_lengths(frames_host, n_utt, 0, T);
+        if (rc) return rc;
+        if (!frames) return fail(DISCO_ERR_INVALID, "null pointer");
+    }
     a.mask = mask;
     a.R0ss = (const float2*)R0ss;
     a.R0nn = (const float2*)R0nn;
@@ -591,13 +598,33 @@ int disco_scm_recursive(const void* Y, const void* Z, const float* mask, const v
     }
     a.lam_block = (float)pow(lambda_cor, block);
     a.lam_last = (float)pow(lambda_cor, T - (a.J - 1) * block);
+    a.frames = frames_host ? frames : nullptr;
+    for (int n = 1; n <= block; ++n) a.lam_n[n - 1] = (float)pow(lambda_cor, n);   // as lam_block / lam_last
     CU(launch_scm_recursive(a, (cudaStream_t)stream), "scm_recursive launch");
     return 0;
 }
 
-int disco_filter_sum_blocks(const void* W, int conj_w, const void* Y, const void* Z, void* out, void* resid, int ref,
-                            int block, int lag, int n_utt, int K, int C, int T, int n_fft, const int* node_sel,
-                            int n_sel, void* stream) {
+int disco_scm_recursive(const void* Y, const void* Z, const float* mask, const void* R0ss, const void* R0nn, void* Rss,
+                        void* Rnn, double lambda_cor, int block, int weight_power, int n_utt, int K, int C, int T,
+                        int n_fft, const int* node_sel, int n_sel, void* stream) {
+    return scm_recursive_common(Y, Z, mask, R0ss, R0nn, Rss, Rnn, lambda_cor, block, weight_power, n_utt, K, C, T,
+                                n_fft, node_sel, n_sel, nullptr, nullptr, stream);
+}
+
+int disco_scm_recursive_lengths(const void* Y, const void* Z, const float* mask, const void* R0ss, const void* R0nn,
+                                void* Rss, void* Rnn, double lambda_cor, int block, int weight_power, int n_utt, int K,
+                                int C, int T, int n_fft, const int* node_sel, int n_sel, const int* frames,
+                                const int* frames_host, void* stream) {
+    if (!frames_host) return fail(DISCO_ERR_INVALID, "null pointer");
+    return scm_recursive_common(Y, Z, mask, R0ss, R0nn, Rss, Rnn, lambda_cor, block, weight_power, n_utt, K, C, T,
+                                n_fft, node_sel, n_sel, frames, frames_host, stream);
+}
+
+// disco_filter_sum_blocks and, with frames / frames_host, disco_filter_sum_blocks_lengths
+static int filter_sum_blocks_common(const void* W, int conj_w, const void* Y, const void* Z, void* out, void* resid,
+                                    int ref, int block, int lag, int n_utt, int K, int C, int T, int n_fft,
+                                    const int* node_sel, int n_sel, const int* frames, const int* frames_host,
+                                    void* stream) {
     OnlineFilterArgs a;
     memset(&a, 0, sizeof(a));
     int rc = make_cat(&a.in, Y, Z, n_utt, K, C, T, n_fft, node_sel, n_sel);
@@ -606,6 +633,11 @@ int disco_filter_sum_blocks(const void* W, int conj_w, const void* Y, const void
     if (!W || !out) return fail(DISCO_ERR_INVALID, "null pointer");
     if (block < 1 || block > 64 || lag < 0) return fail(DISCO_ERR_INVALID, "bad block / lag");
     if (ref < 0 || ref >= C + K - 1) return fail(DISCO_ERR_INVALID, "ref channel out of range");
+    if (frames_host) {
+        rc = check_lengths(frames_host, n_utt, 0, T);
+        if (rc) return rc;
+        if (!frames) return fail(DISCO_ERR_INVALID, "null pointer");
+    }
     a.W = (const float2*)W;
     a.conj_w = conj_w;
     a.out = (float2*)out;
@@ -614,8 +646,25 @@ int disco_filter_sum_blocks(const void* W, int conj_w, const void* Y, const void
     a.P = block;
     a.J = (T + block - 1) / block;
     a.lag = lag;
+    a.frames = frames_host ? frames : nullptr;
     CU(launch_filter_sum_blocks(a, (cudaStream_t)stream), "filter_sum_blocks launch");
     return 0;
+}
+
+int disco_filter_sum_blocks(const void* W, int conj_w, const void* Y, const void* Z, void* out, void* resid, int ref,
+                            int block, int lag, int n_utt, int K, int C, int T, int n_fft, const int* node_sel,
+                            int n_sel, void* stream) {
+    return filter_sum_blocks_common(W, conj_w, Y, Z, out, resid, ref, block, lag, n_utt, K, C, T, n_fft, node_sel,
+                                    n_sel, nullptr, nullptr, stream);
+}
+
+int disco_filter_sum_blocks_lengths(const void* W, int conj_w, const void* Y, const void* Z, void* out, void* resid,
+                                    int ref, int block, int lag, int n_utt, int K, int C, int T, int n_fft,
+                                    const int* node_sel, int n_sel, const int* frames, const int* frames_host,
+                                    void* stream) {
+    if (!frames_host) return fail(DISCO_ERR_INVALID, "null pointer");
+    return filter_sum_blocks_common(W, conj_w, Y, Z, out, resid, ref, block, lag, n_utt, K, C, T, n_fft, node_sel,
+                                    n_sel, frames, frames_host, stream);
 }
 
 int disco_stream_stft(const float* hist, const float* chunk, float* hist_out, void* Y, void* Y_blk, int n_sig,

@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <type_traits>
 
 namespace disco {
 
@@ -193,10 +194,20 @@ struct OnlineArgs {
     float lam_block, lam_last;   // lambda^P, lambda^(frames of the last block)
     float gw[64];           // (1 - lambda) lambda^k, k = 0..P-1
 };
-cudaError_t launch_scm_recursive(const OnlineArgs& a, cudaStream_t st);
+// Utterances of their own lengths: the kernels' template LEN = true take this struct, LEN = false the plain
+// OnlineArgs, so the uniform kernels keep their parameter layout.  Utterance b = grp / n_sel has frames[b] <= T
+// frames and J_b = ceil(frames[b] / P) blocks; its short last block decays by lam_n[frames - 1]; blocks >= J_b are
+// stored as 0.  frames = null runs the uniform kernels.
+struct OnlineLengthsArgs : OnlineArgs {
+    const int* frames;      // [n_utt] device, or null
+    float lam_n[64];        // (float)lambda^n, n = 1..P (lam_n[P - 1] = lam_block)
+};
+template <bool LEN>
+using OnlineParams = std::conditional_t<LEN, OnlineLengthsArgs, OnlineArgs>;
+cudaError_t launch_scm_recursive(const OnlineLengthsArgs& a, cudaStream_t st);
 // D = 9..16 (online_wide.cu): a CTA per (group, 32-bin block) streams the frames and carries R_(j-1) itself; same
 // values as launch_scm_recursive's two-level scan.  Reads of R0: upper triangle, real part of the diagonal.
-cudaError_t launch_scm_recursive_wide(const OnlineArgs& a, cudaStream_t st);
+cudaError_t launch_scm_recursive_wide(const OnlineLengthsArgs& a, cudaStream_t st);
 
 struct OnlineFilterArgs {
     CatArgs in;
@@ -205,7 +216,11 @@ struct OnlineFilterArgs {
     float2* out;            // [n_grp][T][F]
     float2* resid;          // optional x[ref] - out
     int ref, P, J, lag;     // frame t uses filter t / P - lag (pass-through of channel `ref` while that is < 0)
+    // utterances of their own lengths, or null: utterance b = grp / n_sel has frames[b] <= T frames; frames from
+    // frames[b] on are written 0 and the filters of blocks >= ceil(frames[b] / P) are never read
+    const int* frames;      // [n_utt] device
 };
+// a.frames selects the length-aware instantiations (template LEN = true); null runs the uniform kernels
 cudaError_t launch_filter_sum_blocks(const OnlineFilterArgs& a, cudaStream_t st);
 cudaError_t launch_filter_sum_blocks_wide(const OnlineFilterArgs& a, cudaStream_t st);   // D = 9..16
 

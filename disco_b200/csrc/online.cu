@@ -11,6 +11,10 @@
 // the batched solver (solve.cu / solve_small.cu) turns into one filter per block, and
 //   filter_sum_blocks   applies filter j(t) = t / P - lag to frame t  (lag = 1: strictly causal, the filter of
 //                the last COMPLETED block; frames before the first filter pass the reference channel through).
+// With a.frames set (template LEN = true) utterance b = grp / n_sel has its own T_b <= T frames and J_b blocks: block
+// j ends at min((j + 1) P, T_b), a short last block decays by lam_n[frames - 1] (the same float as a run of that
+// utterance alone), nothing past T_b is read, and blocks >= J_b / frames >= T_b are written as exact zeros.  Every
+// (group, block, bin) entry then equals the utterance run alone bit for bit.  LEN = false is the uniform kernel.
 #include "kernels.h"
 #include "scm_core.cuh"
 
@@ -18,15 +22,17 @@ namespace disco {
 
 constexpr int kOnlineBY = 4;   // blocks of frames per CTA (threadIdx.y)
 
-template <int D>
-__global__ void __launch_bounds__(32 * kOnlineBY) scm_blocks_kernel(OnlineArgs a) {
+template <int D, bool LEN>
+__global__ void __launch_bounds__(32 * kOnlineBY) scm_blocks_kernel(OnlineParams<LEN> a) {
     using G = PairGeom<D, 1>;
     const int T = a.in.T, F = a.in.F;
     const int f = blockIdx.x * 32 + threadIdx.x;
     const int j = blockIdx.y * kOnlineBY + threadIdx.y;
     const int grp = blockIdx.z;
     if (f >= F || j >= a.J) return;
-    const int t0 = j * a.P, t1 = min(T, t0 + a.P);          // frames [t0, t1)
+    int Tn = T;                                             // frames of this group's utterance
+    if constexpr (LEN) Tn = a.frames[grp / a.in.n_sel];
+    const int t0 = j * a.P, t1 = min(Tn, t0 + a.P);         // frames [t0, t1): none past the end (A_j = 0 stored)
     const float2* ch[D];
 #pragma unroll
     for (int d = 0; d < D; ++d) ch[d] = cat_channel(a.in, grp, d) + f;
@@ -53,7 +59,8 @@ __global__ void __launch_bounds__(32 * kOnlineBY) scm_blocks_kernel(OnlineArgs a
 }
 
 // R_j = lam_j R_(j-1) + A_j in place, one thread per (group, bin, entry); R_(-1) = R0 (or 0)
-__global__ void scm_combine_kernel(OnlineArgs a, int DD) {
+template <bool LEN>
+__global__ void scm_combine_kernel(OnlineParams<LEN> a, int DD) {
     const size_t per_grp = (size_t)a.in.F * DD;
     const size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= per_grp) return;
@@ -65,6 +72,17 @@ __global__ void scm_combine_kernel(OnlineArgs a, int DD) {
     for (int w = 0; w < 2; ++w) {
         float2 r = init[w] ? init[w][(size_t)grp * per_grp + e] : make_float2(0.f, 0.f);
         float2* p = mats[w] + (size_t)grp * a.J * per_grp + e;
+        if constexpr (LEN) {   // this utterance's J_b blocks (the later ones keep the zeros of scm_blocks)
+            const int Tn = a.frames[grp / a.in.n_sel], Jn = (Tn + a.P - 1) / a.P;
+            const float lam_end = a.lam_n[Tn - (Jn - 1) * a.P - 1];
+            for (int j = 0; j < Jn; ++j) {
+                const float lam = j == Jn - 1 ? lam_end : a.lam_block;
+                const float2 v = p[(size_t)j * per_grp];
+                r = make_float2(fmaf(lam, r.x, v.x), fmaf(lam, r.y, v.y));
+                p[(size_t)j * per_grp] = r;
+            }
+            continue;
+        }
         for (int j = 0; j < a.J; ++j) {
             const float lam = (j == a.J - 1 && last != a.P) ? a.lam_last : a.lam_block;
             const float2 v = p[(size_t)j * per_grp];
@@ -74,14 +92,25 @@ __global__ void scm_combine_kernel(OnlineArgs a, int DD) {
     }
 }
 
-template <int D>
+template <int D, bool LEN>
 __global__ void __launch_bounds__(32 * kOnlineBY) filter_sum_blocks_kernel(OnlineFilterArgs a) {
     const int T = a.in.T, F = a.in.F;
     const int f = blockIdx.x * 32 + threadIdx.x;
     const int j = blockIdx.y * kOnlineBY + threadIdx.y;
     const int grp = blockIdx.z;
     if (f >= F || j >= a.J) return;
-    const int t0 = j * a.P, t1 = min(T, t0 + a.P);
+    const int t0 = j * a.P;
+    int t1 = min(T, t0 + a.P);
+    if constexpr (LEN) {   // frames past the utterance's end are 0, and neither x nor W is read for them
+        const int Tn = a.frames[grp / a.in.n_sel];
+        for (int t = max(t0, Tn); t < t1; ++t) {
+            const size_t o = ((size_t)grp * T + t) * F + f;
+            a.out[o] = make_float2(0.f, 0.f);
+            if (a.resid) a.resid[o] = make_float2(0.f, 0.f);
+        }
+        if (t0 >= Tn) return;                               // block j >= J_b: its filter jw < j is never needed
+        t1 = min(t1, Tn);
+    }
     const int jw = j - a.lag;                               // filter in force during block j
     float2 w[D];
 #pragma unroll
@@ -111,25 +140,29 @@ __global__ void __launch_bounds__(32 * kOnlineBY) filter_sum_blocks_kernel(Onlin
 }
 
 template <int D>
-static cudaError_t launch_blocks_d(const OnlineArgs& a, cudaStream_t st) {
+static cudaError_t launch_blocks_d(const OnlineLengthsArgs& a, cudaStream_t st) {
     dim3 grid((a.in.F + 31) / 32, (a.J + kOnlineBY - 1) / kOnlineBY, a.in.n_grp), block(32, kOnlineBY);
-    scm_blocks_kernel<D><<<grid, block, 0, st>>>(a);
+    const OnlineArgs& u = a;   // the uniform kernels' parameters
+    if (a.frames) scm_blocks_kernel<D, true><<<grid, block, 0, st>>>(a);
+    else scm_blocks_kernel<D, false><<<grid, block, 0, st>>>(u);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     const size_t per_grp = (size_t)a.in.F * D * D;
     dim3 grid2((unsigned)((per_grp + 255) / 256), a.in.n_grp);
-    scm_combine_kernel<<<grid2, 256, 0, st>>>(a, D * D);
+    if (a.frames) scm_combine_kernel<true><<<grid2, 256, 0, st>>>(a, D * D);
+    else scm_combine_kernel<false><<<grid2, 256, 0, st>>>(u, D * D);
     return cudaGetLastError();
 }
 
 template <int D>
 static cudaError_t launch_filter_d(const OnlineFilterArgs& a, cudaStream_t st) {
     dim3 grid((a.in.F + 31) / 32, (a.J + kOnlineBY - 1) / kOnlineBY, a.in.n_grp), block(32, kOnlineBY);
-    filter_sum_blocks_kernel<D><<<grid, block, 0, st>>>(a);
+    if (a.frames) filter_sum_blocks_kernel<D, true><<<grid, block, 0, st>>>(a);
+    else filter_sum_blocks_kernel<D, false><<<grid, block, 0, st>>>(a);
     return cudaGetLastError();
 }
 
-cudaError_t launch_scm_recursive(const OnlineArgs& a, cudaStream_t st) {
+cudaError_t launch_scm_recursive(const OnlineLengthsArgs& a, cudaStream_t st) {
     switch (a.in.C + a.in.K - 1) {
         case 1: return launch_blocks_d<1>(a, st);
         case 2: return launch_blocks_d<2>(a, st);

@@ -18,6 +18,10 @@
 // The Nyquist block of F = 32n + 1 keeps lane 0 on bin F - 1 and leaves the other 31 lanes idle (their copies are
 // zero-filled, nothing is read or stored): a lane butterfly or lanes mapped to blocks would change the order of the
 // sums, and an idle-lane CTA takes no longer than a full one.
+//
+// LEN = true (a.frames set): the group's utterance has its own Tn <= T frames.  The ring streams frames [0, Tn) only,
+// the last block closes at Tn - 1 with lam_n[frames - 1], and the blocks past it are stored as exact zeros: the same
+// frames, tiles and operations as a call on that utterance alone, so the same bits.
 #include "kernels.h"
 #include "scm_core.cuh"
 
@@ -35,12 +39,18 @@ struct OnlineWideCfg {
 };
 
 // block j closes: R_j = lam_j R_(j-1) + A_j on this partition's pairs (R_(-1) = R0 or 0), stored with mirrors
-template <int D, int PART>
-DISCO_DEV void online_close(const OnlineArgs& a, int grp, int f, int j, float2 (&ps)[PairGeom<D, 4>::NPP],
-                            float2 (&pn)[PairGeom<D, 4>::NPP]) {
+template <int D, int PART, bool LEN>
+DISCO_DEV void online_close(const OnlineParams<LEN>& a, int grp, int f, int j, int Tn,
+                            float2 (&ps)[PairGeom<D, 4>::NPP], float2 (&pn)[PairGeom<D, 4>::NPP]) {
     using G = PairGeom<D, 4>;
     const int F = a.in.F;
-    const float lam = (j == a.J - 1 && a.in.T - j * a.P != a.P) ? a.lam_last : a.lam_block;
+    float lam;
+    if constexpr (LEN) {   // the utterance's last block may be short: lambda^(its frames)
+        const int n = min(Tn - j * a.P, a.P);
+        lam = a.lam_n[n - 1];
+    } else {
+        lam = (j == a.J - 1 && a.in.T - j * a.P != a.P) ? a.lam_last : a.lam_block;
+    }
     const float2 *cs = nullptr, *cn = nullptr;
     if (j > 0) {   // this thread's own store of block j - 1
         const size_t prev = ((size_t)(grp * a.J + j - 1) * F + f) * D * D;
@@ -71,9 +81,9 @@ DISCO_DEV void online_close(const OnlineArgs& a, int grp, int f, int j, float2 (
 }
 
 // one warp's pass over the ns frames [t, t + ns) of a stage; closes every block whose last frame is among them
-template <int D, int TS, int PART>
-DISCO_DEV void online_tile(const OnlineArgs& a, const float2* yb, const float* mb, bool has_mask, int grp, int f,
-                           bool ok, int t, int ns, int& j, int& t1, float2 (&ps)[PairGeom<D, 4>::NPP],
+template <int D, int TS, int PART, bool LEN>
+DISCO_DEV void online_tile(const OnlineParams<LEN>& a, const float2* yb, const float* mb, bool has_mask, int grp, int f,
+                           bool ok, int t, int ns, int Tn, int& j, int& t1, float2 (&ps)[PairGeom<D, 4>::NPP],
                            float2 (&pn)[PairGeom<D, 4>::NPP]) {
     using G = PairGeom<D, 4>;
 #pragma unroll 1
@@ -90,17 +100,17 @@ DISCO_DEV void online_tile(const OnlineArgs& a, const float2* yb, const float* m
         const float wn = !has_mask ? 0.f : (a.power == 2 ? (1.f - m) * (1.f - m) : 1.f - m);
         WidePairAcc<D, 4, PART>::run(x, xs, g * ws, g * wn, ps, pn);
         if (t == t1 - 1) {
-            if (ok) online_close<D, PART>(a, grp, f, j, ps, pn);
+            if (ok) online_close<D, PART, LEN>(a, grp, f, j, Tn, ps, pn);
 #pragma unroll
             for (int q = 0; q < G::NPP; ++q) ps[q] = pn[q] = make_float2(0.f, 0.f);
             ++j;
-            t1 = min(a.in.T, t1 + a.P);
+            t1 = min(LEN ? Tn : a.in.T, t1 + a.P);
         }
     }
 }
 
-template <int D, int TS, int NS, int MINB>
-__global__ void __launch_bounds__(32 * 4, MINB) scm_recursive_wide_kernel(OnlineArgs a) {
+template <int D, int TS, int NS, int MINB, bool LEN>
+__global__ void __launch_bounds__(32 * 4, MINB) scm_recursive_wide_kernel(OnlineParams<LEN> a) {
     using G = OnlineWideCfg<D, TS, NS>;
     extern __shared__ __align__(16) unsigned char online_smem[];
     float2* const ystage = reinterpret_cast<float2*>(online_smem);
@@ -112,7 +122,9 @@ __global__ void __launch_bounds__(32 * 4, MINB) scm_recursive_wide_kernel(Online
     const int f = blockIdx.x * 32 + lane;
     const bool ok = f < F;                           // lanes past F (31 of the Nyquist block) stay idle
     const int fcol = ok ? f : F - 1;
-    const int ntile = (T + TS - 1) / TS;
+    int Tn = T;                                      // frames of this group's utterance (T: the row stride)
+    if constexpr (LEN) Tn = a.frames[grp / a.in.n_sel];
+    const int ntile = (Tn + TS - 1) / TS;
     const bool has_mask = a.mask != nullptr;
 
     if (threadIdx.x < D) plane[threadIdx.x] = cat_channel(a.in, grp, threadIdx.x);
@@ -123,7 +135,7 @@ __global__ void __launch_bounds__(32 * 4, MINB) scm_recursive_wide_kernel(Online
         if (i < ntile) {
             const int st = i % NS;
             const int t = i * TS + warp;             // warp w copies frame slot w of every channel
-            const bool v = ok && t < T;
+            const bool v = ok && t < Tn;
             const size_t toff = (size_t)(v ? t : 0) * F + fcol;
             float2* dst = ystage + (st * G::YROWS + warp) * 32 + lane;
 #pragma unroll
@@ -136,7 +148,7 @@ __global__ void __launch_bounds__(32 * 4, MINB) scm_recursive_wide_kernel(Online
     float2 ps[G::NPP], pn[G::NPP];
 #pragma unroll
     for (int q = 0; q < G::NPP; ++q) ps[q] = pn[q] = make_float2(0.f, 0.f);
-    int j = 0, t1 = min(T, a.P);                     // current block and its end
+    int j = 0, t1 = min(Tn, a.P);                    // current block and its end
 
 #pragma unroll
     for (int i = 0; i < NS - 1; ++i) issue(i);
@@ -146,30 +158,44 @@ __global__ void __launch_bounds__(32 * 4, MINB) scm_recursive_wide_kernel(Online
         issue(i + NS - 1);
         const float2* yb = ystage + (i % NS) * G::YROWS * 32 + lane;
         const float* mb = mstage + (i % NS) * TS * 32 + lane;
-        const int t0 = i * TS, ns = min(TS, T - t0);
+        const int t0 = i * TS, ns = min(TS, Tn - t0);
         switch (warp) {   // warp-uniform: keeps the (i, j) of every accumulator compile-time
-            case 0: online_tile<D, TS, 0>(a, yb, mb, has_mask, grp, f, ok, t0, ns, j, t1, ps, pn); break;
-            case 1: online_tile<D, TS, 1>(a, yb, mb, has_mask, grp, f, ok, t0, ns, j, t1, ps, pn); break;
-            case 2: online_tile<D, TS, 2>(a, yb, mb, has_mask, grp, f, ok, t0, ns, j, t1, ps, pn); break;
-            default: online_tile<D, TS, 3>(a, yb, mb, has_mask, grp, f, ok, t0, ns, j, t1, ps, pn); break;
+            case 0: online_tile<D, TS, 0, LEN>(a, yb, mb, has_mask, grp, f, ok, t0, ns, Tn, j, t1, ps, pn); break;
+            case 1: online_tile<D, TS, 1, LEN>(a, yb, mb, has_mask, grp, f, ok, t0, ns, Tn, j, t1, ps, pn); break;
+            case 2: online_tile<D, TS, 2, LEN>(a, yb, mb, has_mask, grp, f, ok, t0, ns, Tn, j, t1, ps, pn); break;
+            default: online_tile<D, TS, 3, LEN>(a, yb, mb, has_mask, grp, f, ok, t0, ns, Tn, j, t1, ps, pn); break;
+        }
+    }
+    if constexpr (LEN) {   // blocks past the utterance's end: exact zeros (this CTA's bins are contiguous per block)
+        const int n = min(32, F - (int)blockIdx.x * 32) * D * D;
+        for (int jj = (Tn + a.P - 1) / a.P; jj < a.J; ++jj) {
+            const size_t mat = ((size_t)(grp * a.J + jj) * F + blockIdx.x * 32) * D * D;
+            for (int e = threadIdx.x; e < n; e += blockDim.x) a.Rss[mat + e] = a.Rnn[mat + e] = make_float2(0.f, 0.f);
         }
     }
 }
 
 template <int D>
-static cudaError_t launch_recursive_wide_d(const OnlineArgs& a, cudaStream_t st) {
+static cudaError_t launch_recursive_wide_d(const OnlineLengthsArgs& a, cudaStream_t st) {
     constexpr int TS = 4, NS = 4;
     constexpr int MINB = 1;
     using G = OnlineWideCfg<D, TS, NS>;
-    auto kern = scm_recursive_wide_kernel<D, TS, NS, MINB>;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G::SMEM);
-    if (e != cudaSuccess) return e;
     dim3 grid((a.in.F + 31) / 32, a.in.n_grp);
-    kern<<<grid, 32 * 4, G::SMEM, st>>>(a);
+    if (a.frames) {
+        auto kern = scm_recursive_wide_kernel<D, TS, NS, MINB, true>;
+        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G::SMEM);
+        if (e != cudaSuccess) return e;
+        kern<<<grid, 32 * 4, G::SMEM, st>>>(a);
+    } else {
+        auto kern = scm_recursive_wide_kernel<D, TS, NS, MINB, false>;
+        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G::SMEM);
+        if (e != cudaSuccess) return e;
+        kern<<<grid, 32 * 4, G::SMEM, st>>>(static_cast<const OnlineArgs&>(a));
+    }
     return cudaGetLastError();
 }
 
-cudaError_t launch_scm_recursive_wide(const OnlineArgs& a, cudaStream_t st) {
+cudaError_t launch_scm_recursive_wide(const OnlineLengthsArgs& a, cudaStream_t st) {
     switch (a.in.C + a.in.K - 1) {
         case 9: return launch_recursive_wide_d<9>(a, st);
         case 10: return launch_recursive_wide_d<10>(a, st);

@@ -492,12 +492,16 @@ def istft_lengths(Y, lengths, length, n_fft=512):
 
 
 @_on_device
-def scm_recursive(Y, mask, Z=None, lambda_cor=0.95, block=8, power=2, R0=None, n_fft=512, node_sel=None):
+def scm_recursive(Y, mask, Z=None, lambda_cor=0.95, block=8, power=2, R0=None, n_fft=512, node_sel=None,
+                  frames=None):
     """Exponentially smoothed SCM pair, R <- lambda R + (1 - lambda) w x x^H per frame (reference
     spatial_correlation_matrix, internal_formulas.py:84-103), sampled after every block of `block` frames.
     Y [B, Ksel, C, T, F], Z [B, K, T, F] or None, mask [B, Ksel, T, F] or None, R0 = (R0ss, R0nn) [B, Ksel, F, D, D]
     -> Rss, Rnn [B, Ksel, J, F, D, D], J = ceil(T / block), D = C + K - 1 <= 16.  At D >= 9 only the upper triangle
-    and the real diagonal of R0 are read (R0 is Hermitian); the values are those of the D <= 8 two-level scan."""
+    and the real diagonal of R0 are read (R0 is Hermitian); the values are those of the D <= 8 two-level scan.
+    frames: None, or host integers, one per utterance in [1, T]: utterance b then has frames[b] frames, its blocks
+    j < ceil(frames[b] / block) equal the call on Y[b, ..., :frames[b], :] alone bit for bit, its later blocks are 0,
+    and no frame from frames[b] on is read."""
     n_utt, K, sel, n_sel, _ = _cat_args(Y, Z, node_sel)
     if mask is not None:
         _need(mask, torch.float32, "mask")
@@ -515,16 +519,25 @@ def scm_recursive(Y, mask, Z=None, lambda_cor=0.95, block=8, power=2, R0=None, n
             _need(r, torch.complex64, "R0")
             if tuple(r.shape) != (B, Ks, F, D, D):
                 raise ValueError("R0 shape %s, expected %s" % (tuple(r.shape), (B, Ks, F, D, D)))
-    _lib.check(_lib.load().disco_scm_recursive(_ptr(Y), _ptr(Z), _ptr(mask), _ptr(r0s), _ptr(r0n), _ptr(Rss), _ptr(Rnn),
-                                               float(lambda_cor), int(block), int(power), n_utt, K, C, T, n_fft, sel,
-                                               n_sel, _stream()))
+    if frames is None:
+        _lib.check(_lib.load().disco_scm_recursive(_ptr(Y), _ptr(Z), _ptr(mask), _ptr(r0s), _ptr(r0n), _ptr(Rss),
+                                                   _ptr(Rnn), float(lambda_cor), int(block), int(power), n_utt, K, C,
+                                                   T, n_fft, sel, n_sel, _stream()))
+    else:
+        dev, hp = _lengths_args(signal_lengths(frames, (B, n_utt // B), T), Y.device)   # n_utt = B * Ksel if Z is None
+        _lib.check(_lib.load().disco_scm_recursive_lengths(_ptr(Y), _ptr(Z), _ptr(mask), _ptr(r0s), _ptr(r0n),
+                                                           _ptr(Rss), _ptr(Rnn), float(lambda_cor), int(block),
+                                                           int(power), n_utt, K, C, T, n_fft, sel, n_sel, _ptr(dev),
+                                                           hp, _stream()))
     return Rss, Rnn
 
 
 @_on_device
-def filter_sum_blocks(W, Y, Z=None, block=8, lag=1, conj=True, ref=0, n_fft=512, node_sel=None):
+def filter_sum_blocks(W, Y, Z=None, block=8, lag=1, conj=True, ref=0, n_fft=512, node_sel=None, frames=None):
     """One filter per block of frames: out[t] = W[t // block - lag]^H x[t] (pass-through of channel `ref` while no
-    filter exists yet).  W [B, Ksel, J, F, D], D = C + K - 1 <= 16 -> out, resid = x[ref] - out, [B, Ksel, T, F]."""
+    filter exists yet).  W [B, Ksel, J, F, D], D = C + K - 1 <= 16 -> out, resid = x[ref] - out, [B, Ksel, T, F].
+    frames: None, or host integers, one per utterance in [1, T]: frames t < frames[b] of utterance b are the call on
+    its first frames[b] frames alone (reading only W[b, :, :ceil(frames[b] / block)]); later frames are 0."""
     _need(W, torch.complex64, "W")
     n_utt, K, sel, n_sel, _ = _cat_args(Y, Z, node_sel)
     B, Ks, C, T, F = Y.shape
@@ -533,9 +546,15 @@ def filter_sum_blocks(W, Y, Z=None, block=8, lag=1, conj=True, ref=0, n_fft=512,
         raise ValueError("W shape %s, expected %s" % (tuple(W.shape), (B, Ks, J, F, D)))
     out = torch.empty((B, Ks, T, F), dtype=torch.complex64, device=Y.device)
     resid = torch.empty_like(out)
-    _lib.check(_lib.load().disco_filter_sum_blocks(_ptr(W), 1 if conj else 0, _ptr(Y), _ptr(Z), _ptr(out), _ptr(resid),
-                                                   int(ref), int(block), int(lag), n_utt, K, C, T, n_fft, sel, n_sel,
-                                                   _stream()))
+    if frames is None:
+        _lib.check(_lib.load().disco_filter_sum_blocks(_ptr(W), 1 if conj else 0, _ptr(Y), _ptr(Z), _ptr(out),
+                                                       _ptr(resid), int(ref), int(block), int(lag), n_utt, K, C, T,
+                                                       n_fft, sel, n_sel, _stream()))
+    else:
+        dev, hp = _lengths_args(signal_lengths(frames, (B, n_utt // B), T), Y.device)   # n_utt = B * Ksel if Z is None
+        _lib.check(_lib.load().disco_filter_sum_blocks_lengths(_ptr(W), 1 if conj else 0, _ptr(Y), _ptr(Z), _ptr(out),
+                                                               _ptr(resid), int(ref), int(block), int(lag), n_utt, K,
+                                                               C, T, n_fft, sel, n_sel, _ptr(dev), hp, _stream()))
     return out, resid
 
 

@@ -261,6 +261,24 @@ DISCO_API int disco_scm_recursive(const void* Y, const void* Z, const float* mas
 DISCO_API int disco_filter_sum_blocks(const void* W, int conj_w, const void* Y, const void* Z, void* out, void* resid,
                      int ref, int block, int lag, int n_utt, int K, int C, int T, int n_fft, const int* node_sel,
                      int n_sel, void* stream);
+/* The same two calls on utterances of their own lengths: utterance b (every node of it) has frames[b] frames,
+ * 1 <= frames[b] <= T, and J_b = ceil(frames[b] / block) blocks; Y, Z and the mask keep their T-frame rows.
+ * disco_scm_recursive_lengths: blocks j < J_b are disco_scm_recursive of that utterance alone (its frames [0,
+ *   frames[b]) as a call with T = frames[b]) bit for bit -- the last block ends at frames[b] and decays by
+ *   lambda^(its frames) -- and blocks J_b .. J - 1 are exact zeros.  No frame >= frames[b] of Y, Z or the mask is
+ *   read.  R0 of the utterance (if given) is used as is, as block -1 of its scan.
+ * disco_filter_sum_blocks_lengths: frames t < frames[b] are disco_filter_sum_blocks of that utterance alone and read
+ *   only the filters of blocks < J_b; frames t >= frames[b] of out and resid are exact zeros, and neither Y / Z nor
+ *   W is read for them.
+ * `frames` is the device copy the kernels read; `frames_host` the same values in host memory, checked before
+ * anything is launched (DISCO_ERR_INVALID for a count out of range or a NULL pointer). */
+DISCO_API int disco_scm_recursive_lengths(const void* Y, const void* Z, const float* mask, const void* R0ss,
+                     const void* R0nn, void* Rss, void* Rnn, double lambda_cor, int block, int weight_power, int n_utt,
+                     int K, int C, int T, int n_fft, const int* node_sel, int n_sel, const int* frames,
+                     const int* frames_host, void* stream);
+DISCO_API int disco_filter_sum_blocks_lengths(const void* W, int conj_w, const void* Y, const void* Z, void* out,
+                     void* resid, int ref, int block, int lag, int n_utt, int K, int C, int T, int n_fft,
+                     const int* node_sel, int n_sel, const int* frames, const int* frames_host, void* stream);
 
 /* ---- streaming STFT / iSTFT (the online Tango session, disco_b200/stream.py) -------------------------
  * disco_stft and disco_istft of signals that arrive chunk by chunk, equal to the whole-signal calls value for value

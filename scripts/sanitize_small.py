@@ -81,3 +81,18 @@ out = tango_batched(torch.from_numpy(y).to(dev), torch.from_numpy(s).to(dev), to
 td = post.to_time(out, 9000, lengths=[9000, 5001, 7003])
 torch.cuda.synchronize()
 print("ok lengths stoi / tango", d.tolist(), float(td["yf"].abs().mean()))
+# online Tango on utterances of their own lengths: block edges, a one-block utterance, the staged wide scan (D = 9)
+# with a block straddling its ring, R0, and filters / masks never read past each utterance's end
+for (B, K, C, L, n_fft, block) in ((3, 1, 4, 6000, 512, 8), (3, 8, 2, 5000, 256, 5), (2, 1, 10, 4000, 1024, 1)):
+    y, _, _ = make_batch(B, K, C, L, seed0=3)
+    H = n_fft // 2
+    lengths = [L, H + 1, 2 * block * H + 7][:B]
+    T, F = 1 + L // H, H + 1
+    masks = (torch.rand(B, K, T, F, device=dev), torch.rand(B, K, T, F, device=dev))
+    R0 = None
+    if K == 1:
+        R0 = tuple(torch.eye(C, dtype=torch.complex64, device=dev).expand(B, K, F, C, C).contiguous() for _ in range(2))
+    out = online.online_tango(torch.from_numpy(y).to(dev), masks, block=block, n_fft=n_fft, R0=R0, lengths=lengths)
+    td = post.to_time(out, L, n_fft=n_fft, names=("yf", "z_y"), layout="TF", lengths=lengths)
+    torch.cuda.synchronize()
+    print("ok online lengths", B, K, C, n_fft, block, float(td["yf"].abs().mean()))
