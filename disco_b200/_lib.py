@@ -70,6 +70,10 @@ SIGNATURES = {
                                   c_int, c_int, c_int, c_int, c_void_p]),
     "disco_stream_istft": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
                                    c_void_p]),
+    "disco_stream_stft_slots": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int_p, c_int, c_int, c_int,
+                                        c_int, c_int, c_int, c_void_p]),
+    "disco_stream_istft_slots": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int_p, c_int, c_int, c_int, c_int,
+                                         c_int, c_void_p]),
     "disco_band_stats": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, ctypes.c_longlong, c_int, c_int,
                                  c_void_p]),
     "disco_bss_eval_workspace": (c_size_t, [c_int, c_int, c_int, c_int, c_int]),

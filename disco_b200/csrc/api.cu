@@ -748,6 +748,96 @@ int disco_stream_istft(const void* Y, float* carry, float* x, int n_sig, int t0,
     return 0;
 }
 
+// disco_stream_stft_slots: the per-slot versions of disco_stream_stft's checks, on the host copy of the records
+int disco_stream_stft_slots(float* hist, const float* chunk, void* Y, void* Y_blk, const int* slots,
+                            const int* slots_host, int n_slot, int n_sig, int n_max, int f_max, int blk_frames,
+                            int n_fft, void* stream) {
+    if (!valid_nfft(n_fft)) return fail(DISCO_ERR_INVALID, "n_fft must be 256, 512 or 1024");
+    if (n_slot <= 0 || n_slot > kMaxGridYZ) return fail(DISCO_ERR_INVALID, "n_slot must be in 1..65535");
+    if (n_sig <= 0 || (n_sig + 1) / 2 > kMaxGridYZ) return fail(DISCO_ERR_INVALID, "n_sig must be in 1..131070");
+    if (n_max < 0 || f_max < 0 || blk_frames < 0) return fail(DISCO_ERR_INVALID, "bad sizes");
+    if (!slots_host || !slots || !hist) return fail(DISCO_ERR_INVALID, "null pointer");
+    const int H = n_fft / 2;
+    for (int s = 0; s < n_slot; ++s) {
+        const int* r = slots_host + (size_t)s * kStftSlotFields;
+        const int length = r[0], n_new = r[1], t0 = r[2], n_fr = r[3], blk_slot = r[4], final_call = r[5];
+        const int sel = r[6];
+        if (n_new < 0 || n_new > n_max || length < n_new || t0 < 0 || n_fr < 0 || n_fr > f_max || (sel != 0 && sel != 1))
+            return fail(DISCO_ERR_INVALID, "bad sizes in a slot record");
+        if ((n_new > 0 && !chunk) || (n_fr > 0 && !Y) || (final_call && n_new > 0))
+            return fail(DISCO_ERR_INVALID, "null pointer (or a chunk on a slot's final call)");
+        const int L0 = length - n_new;
+        if (n_fr > 0) {
+            const int t1 = t0 + n_fr - 1;
+            const bool arrived = length > H && (final_call ? t1 <= length / H : (t1 == 0 || (t1 + 1) * H <= length));
+            if (!arrived || (t0 >= 1 && (t0 - 1) * H < L0 - n_fft))
+                return fail(DISCO_ERR_INVALID, "a slot's frames are not complete, or older than its carried history");
+            if (Y_blk && (blk_slot < 0 || blk_slot + n_fr > blk_frames))
+                return fail(DISCO_ERR_INVALID, "a slot's frames lie outside the block buffer");
+        }
+    }
+    Tables tb;
+    int rc = get_tables(n_fft, &tb);
+    if (rc) return rc;
+    StreamStftSlotsArgs a;
+    memset(&a, 0, sizeof(a));
+    a.hist = hist;
+    a.chunk = chunk;
+    a.Y = (float2*)Y;
+    a.Y_blk = (float2*)Y_blk;
+    a.twiddle = tb.twiddle;
+    a.window = tb.win_half;
+    a.n_sig = n_sig;
+    a.blk_frames = blk_frames;
+    a.slots = slots;
+    a.n_slot = n_slot;
+    a.n_max = n_max;
+    a.f_max = f_max;
+    CU(launch_stream_stft_slots(a, n_fft, (cudaStream_t)stream), "stream_stft_slots launch");
+    return 0;
+}
+
+// disco_stream_istft_slots: the per-slot versions of disco_stream_istft's checks, on the host copy of the records
+int disco_stream_istft_slots(const void* Y, float* carry, float* x, const int* slots, const int* slots_host,
+                             int n_slot, int n_sig, int f_max, int s_max, int n_fft, void* stream) {
+    if (!valid_nfft(n_fft)) return fail(DISCO_ERR_INVALID, "n_fft must be 256, 512 or 1024");
+    if (n_slot <= 0 || n_slot > kMaxGridYZ) return fail(DISCO_ERR_INVALID, "n_slot must be in 1..65535");
+    if (n_sig <= 0 || (n_sig + 1) / 2 > kMaxGridYZ) return fail(DISCO_ERR_INVALID, "n_sig must be in 1..131070");
+    if (f_max < 0 || s_max < 0) return fail(DISCO_ERR_INVALID, "bad sizes");
+    if (!slots_host || !slots || !carry) return fail(DISCO_ERR_INVALID, "null pointer");
+    const int H = n_fft / 2;
+    for (int s = 0; s < n_slot; ++s) {
+        const int* r = slots_host + (size_t)s * kIstftSlotFields;
+        const int t0 = r[0], n_fr = r[1], length = r[2], final_call = r[3], x_first = r[4];
+        if (t0 < 0 || n_fr < 0 || n_fr > f_max || x_first < 0 || (length < 1 && (n_fr > 0 || final_call)))
+            return fail(DISCO_ERR_INVALID, "bad sizes in a slot record");
+        if (n_fr > 0 && !Y) return fail(DISCO_ERR_INVALID, "null pointer");
+        if (n_fr <= 0 && !final_call) continue;   // the slot is not run
+        const int lo = (t0 > 0 ? t0 - 1 : 0) * H;
+        int hi = final_call ? length : (t0 + n_fr - 1) * H;
+        if (hi > length) hi = length;
+        if (hi > lo) {
+            if (!x) return fail(DISCO_ERR_INVALID, "null pointer");
+            if (lo < x_first || hi > x_first + s_max) return fail(DISCO_ERR_INVALID, "a slot's output samples lie outside x");
+        }
+    }
+    Tables tb;
+    int rc = get_tables(n_fft, &tb);
+    if (rc) return rc;
+    IstftArgs a;
+    memset(&a, 0, sizeof(a));
+    a.Y = (const float2*)Y;
+    a.x = x;
+    a.carry = carry;
+    a.twiddle = tb.twiddle;
+    a.window = tb.win;
+    a.n_sig = n_sig;
+    a.y_frames = f_max;
+    a.ld = s_max;
+    CU(launch_stream_istft_slots(a, slots, n_slot, n_fft, (cudaStream_t)stream), "stream_istft_slots launch");
+    return 0;
+}
+
 int disco_band_stats(const float* x, const float* sel, const double* ba, double* stats, int n_sig, int length,
                      long long row_stride, int n_band, int order, void* stream) {
     if (!x || !ba || !stats || n_sig < 1 || length < 1 || n_band < 1 || row_stride < length)

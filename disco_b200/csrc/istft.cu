@@ -218,6 +218,50 @@ __global__ void __launch_bounds__(IGeom<N>::THREADS) istft_lengths_kernel(IstftA
     }
 }
 
+// A pool of independent streams (disco_stream_istft_slots): grid (1, pairs of a slot, slots).  Slot blockIdx.z runs the
+// stream body on its own rows with its record {t0, n_fr, length, final, x_first}, as disco_stream_istft runs it on
+// that slot alone.
+template <int N>
+__global__ void __launch_bounds__(IGeom<N>::THREADS) stream_istft_slots_kernel(IstftArgs p, const int* slots) {
+    constexpr int H = IGeom<N>::H, F = IGeom<N>::F;
+    const int* r = slots + (size_t)blockIdx.z * kIstftSlotFields;
+    const int t0 = r[0], n_fr = r[1];
+    if (n_fr <= 0 && !r[3]) return;   // CTA-uniform: no frames, not the end of the stream
+    IstftArgs q = p;
+    const size_t row0 = (size_t)blockIdx.z * p.n_sig;
+    q.Y = p.Y + row0 * p.y_frames * F;
+    q.x = p.x ? p.x + row0 * p.ld : nullptr;
+    q.carry = p.carry + row0 * H;
+    q.L = r[2];
+    q.y_t0 = t0;
+    q.j_begin = t0;
+    q.j_end = t0 + n_fr;
+    q.fpc = n_fr;
+    q.tail = r[3];
+    q.x_first = r[4];
+    istft_body<N, true>(q);
+}
+
+template <int N>
+static cudaError_t launch_slots_n(const IstftArgs& a, const int* slots, int n_slot, cudaStream_t st) {
+    using G = IGeom<N>;
+    cudaError_t e = cudaFuncSetAttribute(stream_istft_slots_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)G::SMEM);
+    if (e != cudaSuccess) return e;
+    stream_istft_slots_kernel<N><<<dim3(1, (a.n_sig + 1) / 2, n_slot), G::THREADS, G::SMEM, st>>>(a, slots);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_stream_istft_slots(const IstftArgs& a, const int* slots, int n_slot, int n_fft, cudaStream_t st) {
+    if (a.n_sig <= 0 || n_slot <= 0) return cudaSuccess;
+    switch (n_fft) {
+        case 256: return launch_slots_n<256>(a, slots, n_slot, st);
+        case 512: return launch_slots_n<512>(a, slots, n_slot, st);
+        case 1024: return launch_slots_n<1024>(a, slots, n_slot, st);
+        default: return cudaErrorInvalidValue;
+    }
+}
+
 IstftLengthsKernel istft_lengths_kernel_for(int n_fft) {
     switch (n_fft) {
         case 256: return {(const void*)istft_lengths_kernel<256>, IGeom<256>::THREADS, IGeom<256>::SMEM, IGeom<256>::ITEMS};

@@ -339,6 +339,24 @@ struct StreamStftArgs {
     int final_call;         // 1: the stream ends at `length` (reflect padding at the end)
 };
 cudaError_t launch_stream_stft(const StreamStftArgs& a, int n_fft, cudaStream_t st);
+// A pool of independent streams (disco_stream_stft_slots): slot s owns signals [s n_sig, (s + 1) n_sig) and the record
+// slots[s][kStftSlotFields] = {length, n_new, t0, n_fr, blk_slot, final, hist_sel, hist_write}.  The slots kernel
+// takes this struct (stream_stft_kernel keeps StreamStftArgs and its parameter layout).  hist is [2][n_slot][n_sig][N]:
+// slot s reads buffer hist_sel and, with hist_write, writes its samples [length - N, length) to the other buffer;
+// chunk [n_slot][n_sig][n_max], Y [n_slot][n_sig][f_max][F], Y_blk [n_slot][n_sig][blk_frames][F].  The uniform
+// fields n_new, length, t0, n_fr, blk_slot, final_call and hist_out are not read.
+constexpr int kStftSlotFields = 8;
+struct StreamStftSlotsArgs : StreamStftArgs {
+    const int* slots;       // [n_slot][kStftSlotFields] device
+    int n_slot, n_max, f_max;
+};
+cudaError_t launch_stream_stft_slots(const StreamStftSlotsArgs& a, int n_fft, cudaStream_t st);
+// The stream iSTFT of a pool (disco_stream_istft_slots, istft.cu): slot s runs istft_body on its signals [s n_sig,
+// (s + 1) n_sig) with the record slots[s][kIstftSlotFields] = {t0, n_fr, length, final, x_first}.  a: Y [n_slot]
+// [n_sig][y_frames][F], carry [n_slot][n_sig][N/2], x [n_slot][n_sig][ld]; a.n_sig is the signals of one slot.  A slot
+// with n_fr = 0 that is not final returns at once.
+constexpr int kIstftSlotFields = 5;
+cudaError_t launch_stream_istft_slots(const IstftArgs& a, const int* slots, int n_slot, int n_fft, cudaStream_t st);
 
 cudaError_t launch_tf_mask(const float2* S, const float2* Nn, float* M, size_t n, int kind, int power,
                            float thr_lin, cudaStream_t st);

@@ -619,6 +619,79 @@ def stream_istft(Y, carry, t0, length, n_fft=512, final=False, x=None, x_first=0
     return x
 
 
+STFT_SLOT_FIELDS = ("length", "n_new", "t0", "n_fr", "blk_slot", "final", "hist_sel", "hist_write")
+ISTFT_SLOT_FIELDS = ("t0", "n_fr", "length", "final", "x_first")
+
+
+def _records(slots, n_slot, fields, name):
+    """Per-slot records [n_slot, len(fields)] as a contiguous host int32 array."""
+    arr = np.asarray(slots)
+    if arr.dtype.kind not in "iu":
+        raise TypeError("%s must be integers, got %s" % (name, arr.dtype))
+    if tuple(arr.shape) != (n_slot, len(fields)):
+        raise ValueError("%s shape %s, expected (%d, %d): %s" % (name, tuple(arr.shape), n_slot, len(fields),
+                                                                ", ".join(fields)))
+    return np.ascontiguousarray(arr, dtype=np.int32)
+
+
+@_on_device
+def stream_stft_slots(hist, chunk, slots, f_max, n_fft=512, Y_blk=None):
+    """stream_stft on a pool of independent streams, one record per slot (STFT_SLOT_FIELDS): slot s holds the signals
+    chunk[s] ([S, ..., n_max] float32, its new samples at the start of each row).  hist [2, S, ..., n_fft] float32 holds
+    two history buffers: slot s reads buffer hist_sel and, with hist_write, writes its new history to the other one.
+    Y_blk [S, ..., P, F] (optional) receives the frames at rows blk_slot ...  Returns Y [S, ..., f_max, F]: frames t0
+    .. t0 + n_fr - 1 of slot s at rows 0 .. n_fr - 1 (later rows are not written).  Signals are paired inside a slot,
+    so each slot equals stream_stft on that slot alone."""
+    _need(hist, torch.float32, "hist")
+    _need(chunk, torch.float32, "chunk")
+    lead, F = tuple(chunk.shape[:-1]), n_fft // 2 + 1
+    if len(lead) < 1 or tuple(hist.shape) != (2,) + lead + (n_fft,):
+        raise ValueError("hist %s / chunk %s, expected [2, S, ..., %d] / [S, ..., n_max]"
+                         % (tuple(hist.shape), tuple(chunk.shape), n_fft))
+    S = lead[0]
+    n_sig = int(np.prod(lead[1:], dtype=np.int64))
+    P = 0
+    if Y_blk is not None:
+        _need(Y_blk, torch.complex64, "Y_blk")
+        P = Y_blk.shape[-2]
+        if tuple(Y_blk.shape) != lead + (P, F):
+            raise ValueError("Y_blk shape %s, expected %s" % (tuple(Y_blk.shape), lead + (P, F)))
+    host = _records(slots, S, STFT_SLOT_FIELDS, "slots")
+    Y = torch.empty(lead + (int(f_max), F), dtype=torch.complex64, device=hist.device)
+    dev = torch.from_numpy(host).to(hist.device)
+    _lib.check(_lib.load().disco_stream_stft_slots(_ptr(hist), _ptr(chunk) if chunk.numel() else None,
+                                                   _ptr(Y) if Y.numel() else None, _ptr(Y_blk), _ptr(dev),
+                                                   host.ctypes.data_as(_lib.c_int_p), S, n_sig, chunk.shape[-1],
+                                                   int(f_max), P, n_fft, _stream()))
+    return Y
+
+
+@_on_device
+def stream_istft_slots(Y, carry, slots, x, n_fft=512):
+    """stream_istft on a pool of independent streams, one record per slot (ISTFT_SLOT_FIELDS): frames t0 .. t0 + n_fr -
+    1 of slot s are Y[s] [S, ..., f_max, F] rows 0 .. n_fr - 1; carry [S, ..., n_fft // 2] is updated in place; the
+    samples that become final are written to x [S, ..., s_max] at x[s, ..., i - x_first].  A slot with n_fr = 0 that
+    is not final is left as it is.  Each slot equals stream_istft on that slot alone.  Returns x."""
+    _need(Y, torch.complex64, "Y")
+    _need(carry, torch.float32, "carry")
+    _need(x, torch.float32, "x")
+    f_max, F = Y.shape[-2:]
+    H = n_fft // 2
+    lead = tuple(Y.shape[:-2])
+    if F != H + 1 or len(lead) < 1 or tuple(carry.shape) != lead + (H,) or tuple(x.shape[:-1]) != lead:
+        raise ValueError("Y %s / carry %s / x %s, expected [S, ..., f_max, %d] / [S, ..., %d] / [S, ..., s_max]"
+                         % (tuple(Y.shape), tuple(carry.shape), tuple(x.shape), H + 1, H))
+    S = lead[0]
+    n_sig = int(np.prod(lead[1:], dtype=np.int64))
+    host = _records(slots, S, ISTFT_SLOT_FIELDS, "slots")
+    dev = torch.from_numpy(host).to(Y.device)
+    _lib.check(_lib.load().disco_stream_istft_slots(_ptr(Y) if Y.numel() else None, _ptr(carry),
+                                                    _ptr(x) if x.numel() else None, _ptr(dev),
+                                                    host.ctypes.data_as(_lib.c_int_p), S, n_sig, f_max, x.shape[-1],
+                                                    n_fft, _stream()))
+    return x
+
+
 @_on_device
 def band_stats(x, ba, sel=None):
     """IIR filter bank + statistics of every band's output (reference metrics.py:96-110: lfilter, then np.var of

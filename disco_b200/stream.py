@@ -15,6 +15,7 @@ Per push, for every run of newly completed frames (a run never crosses a block b
     mwf_solve            and the block's filters W1_j, W2_j
     stream_istft         the hop blocks of yf that became final (csrc/stream.cu)
 """
+import numpy as np
 import torch
 
 from . import ops
@@ -266,3 +267,343 @@ class OnlineTangoStream:
             return {"t0": T0, "z_y": empty, "zn": empty.clone(), "yf": empty.clone(), "yf_time": yf_time}
         cat = (lambda i: parts[0][i]) if len(parts) == 1 else (lambda i: torch.cat([p[i] for p in parts], dim=2))
         return {"t0": T0, "z_y": cat(0), "zn": cat(1), "yf": cat(2), "yf_time": yf_time}
+
+
+def pool_rounds(T0, T1, block):
+    """The rounds of one call of OnlineTangoPool: slot s completes frames [T0[s], T1[s]); they are cut into runs that
+    never cross a block boundary (multiples of `block`), and round r holds every slot's r-th run.  Returns int64 arrays
+    (t0, n) of shape [R, S]: run r of slot s is frames [t0[r, s], t0[r, s] + n[r, s]); n[r, s] = 0 once slot s has no
+    r-th run, and t0 is then where the slot stands (T1[s])."""
+    T0, T1, P = np.asarray(T0, dtype=np.int64), np.asarray(T1, dtype=np.int64), int(block)
+    if T0.shape != T1.shape or T0.ndim != 1 or P < 1 or np.any(T1 < T0) or np.any(T0 < 0):
+        raise ValueError("need 0 <= T0 <= T1, one entry per slot, and block >= 1")
+    b0 = (T0 // P + 1) * P                                   # the first block boundary after T0
+    runs = np.where(T1 > T0, 1 + np.maximum(T1 - b0 + P - 1, 0) // P, 0)
+    R = int(runs.max()) if runs.size else 0
+    r = np.arange(R, dtype=np.int64)[:, None]
+    start = np.where(r == 0, T0, b0 + (r - 1) * P)
+    n = np.maximum(np.minimum(T1, b0 + r * P) - start, 0)
+    return np.minimum(start, T1), n
+
+
+class OnlineTangoPool:
+    """S slots, each an independent online Tango stream of K nodes x C microphones that opens, advances and closes on
+    its own; the parameters are those of OnlineTangoStream, and one pool has one geometry (D = C + K - 1 <= 16):
+
+        pool = OnlineTangoPool(S, K, C, n_fft=512, lambda_cor=0.95, block=8, lag=1)
+        pool.open(slots, R0=None)        # R0 = (R_ss, R_nn) complex64 [len(slots), K, F, C, C], or None
+        out = pool.push(y, n, mask_fn)   # y [S, K, C, n_max] float32 CUDA; slot s gets y[s, ..., :n[s]]
+        out = pool.close(slots, mask_fn) # the last frame (reflected at the end), the partial block, the last samples
+        pool.filters(slot)               # (W1 [K, F, C], W2 [K, F, D]) of the slot's last closed block, or None
+
+    For every slot, its outputs concatenated over the calls from open to close equal, value for value, those of
+    OnlineTangoStream(1, K, C) fed the same samples (hence online_tango on the slot's whole signal and ops.istft of its
+    yf), with the masks mask_fn returned -- whatever the other slots do, the slot's index, and the cut of its samples
+    into pushes.  A slot's K C signals are paired into transforms inside the slot, as the single stream pairs them.
+
+    mask_fn(t0, n_fr, Y, z_y, zn) -> (mask_z, mask_w) is called once per round: every slot's frames of the call are
+    cut into runs that never cross its block boundary (pool_rounds), and round r holds every slot's r-th run.  t0 and
+    n_fr are host int arrays [S] (n_fr[s] = 0: no frames of slot s in the round); Y is [S, K, C, f_max, F], z_y and zn
+    [S, K, f_max, F]; the masks are float32 [S, K, f_max, F] (mask_w = None means mask_z).  Rows at or past n_fr[s] of
+    Y are not defined, those of z_y and zn are 0, and those of the masks are never read.
+
+    push and close return dict(t0, frames, s0, samples: host int arrays [S]; z_y, zn, yf [S, K, f_max, F]: the frames
+    [t0[s], t0[s] + frames[s]) of slot s, exactly 0 from frames[s] on; yf_time [S, K, s_max]: its samples [s0[s],
+    s0[s] + samples[s]) that became final, exactly 0 after them).  Invalid calls raise ValueError before any work and
+    leave the pool as it was; an exception raised after work has started (by mask_fn, or a mask of the wrong shape)
+    closes the slots the call advanced, and the others stay open and exact."""
+
+    def __init__(self, S, K, C, n_fft=512, lambda_cor=0.95, block=8, lag=1, mu=1.0, rank=1, ref_mic=0, device=None):
+        S, K, C = int(S), int(K), int(C)
+        if S < 1 or K < 1 or C < 1:
+            raise ValueError("S, K and C must be positive")
+        if n_fft not in N_FFTS:
+            raise ValueError("n_fft must be 256, 512 or 1024")
+        if not 1 <= int(block) <= 64:
+            raise ValueError("block must be 1..64 frames")
+        if not 0.0 <= float(lambda_cor) < 1.0:
+            raise ValueError("lambda_cor must be in [0, 1)")
+        if int(lag) == 0:
+            raise NotImplementedError("lag = 0 filters a frame with its own block's statistics, whose masks arrive "
+                                      "only after the block's later frames are out")
+        if int(lag) < 0:
+            raise ValueError("lag must be positive")
+        D = C + K - 1
+        if D > 16:
+            raise NotImplementedError("the pool covers C + K - 1 <= 16 channels, got %d" % D)
+        if not 0 <= int(ref_mic) < C:
+            raise ValueError("ref_mic must be in 0..C-1")
+        if S > 65535:
+            raise ValueError("at most 65535 slots")
+        device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        if device.type != "cuda":
+            raise TypeError("the pool runs on a CUDA device, got %s" % device)
+        if device.index is None:
+            device = torch.device("cuda", torch.cuda.current_device())
+        self.S, self.K, self.C, self.D, self.F = S, K, C, D, n_fft // 2 + 1
+        self.n_fft, self.block, self.lag = n_fft, int(block), int(lag)
+        self.lambda_cor, self.mu, self.rank, self.ref_mic = float(lambda_cor), float(mu), rank, int(ref_mic)
+        self.device = device
+        # host state per slot
+        self._open = np.zeros(S, dtype=bool)
+        self._L = np.zeros(S, dtype=np.int64)          # samples in
+        self._T = np.zeros(S, dtype=np.int64)          # frames out
+        self._S = np.zeros(S, dtype=np.int64)          # time samples out
+        self._par = np.zeros(S, dtype=np.int64)        # which history buffer holds the slot's last n_fft samples
+        self._nclosed = np.zeros(S, dtype=np.int64)    # closed blocks
+        self._bufs = False
+
+    def _alloc(self):
+        """Device state, allocated on the first open."""
+        if self._bufs:
+            return
+        S, K, C, D, F, P, N, dev = self.S, self.K, self.C, self.D, self.F, self.block, self.n_fft, self.device
+        f32, c64 = dict(dtype=torch.float32, device=dev), dict(dtype=torch.complex64, device=dev)
+        self._hist = torch.zeros((2, S, K, C, N), **f32)
+        self._carry = torch.zeros((S, K, N // 2), **f32)
+        # the open block of every slot: its spectra, masks and (K > 1) step-1 outputs
+        self._Yblk = torch.zeros((S, K, C, P, F), **c64)
+        self._m1 = torch.zeros((S, K, P, F), **f32)
+        self._m2 = torch.zeros((S, K, P, F), **f32)
+        self._zblk = torch.zeros((S, K, P, F), **c64) if K > 1 else None
+        # carried statistics (zeros stand for "none yet": the scan's R_(-1) is 0 either way)
+        self._R1 = (torch.zeros((S, K, F, C, C), **c64), torch.zeros((S, K, F, C, C), **c64))
+        self._R2 = (torch.zeros((S, K, F, D, D), **c64), torch.zeros((S, K, F, D, D), **c64))
+        # ring of the last lag + 1 filters: block j's at j % (lag + 1).  Entries of blocks before the first hold the
+        # pass-through of the reference channel, stored as (e_ref, -0) so that the kernel's conjugate is exactly the
+        # weight vector of filter_sum_blocks' own pass-through.
+        self._W1 = torch.zeros((S, self.lag + 1, K, F, C), **c64)
+        self._W2 = torch.zeros((S, self.lag + 1, K, F, D), **c64)
+        self._pass = []
+        for d in (C, D):
+            re = torch.zeros((K, F, d), **f32)
+            re[..., self.ref_mic] = 1.0
+            self._pass.append(torch.complex(re, torch.full_like(re, -0.0)))
+        self._bufs = True
+
+    # ---------------------------------------------------------------- state
+    def is_open(self, slot):
+        return bool(self._open[self._slot_list([slot])[0]])
+
+    @property
+    def samples_in(self):
+        return self._L.copy()
+
+    @property
+    def frames_out(self):
+        return self._T.copy()
+
+    @property
+    def samples_out(self):
+        return self._S.copy()
+
+    def filters(self, slot):
+        """(W1 [K, F, C], W2 [K, F, D]) of the slot's last closed block (in force from block j + lag), or None before
+        its first; kept after close until the slot is opened again."""
+        s = int(self._slot_list([slot])[0])
+        if self._nclosed[s] == 0:
+            return None
+        pos = int((self._nclosed[s] - 1) % (self.lag + 1))
+        return self._W1[s, pos].clone(), self._W2[s, pos].clone()
+
+    # ---------------------------------------------------------------- public calls
+    def open(self, slots, R0=None):
+        """Open free slots: every slot starts a new stream (history, block buffers, filters and iSTFT carry reset; the
+        carried matrices from R0, or zeros).  R0 = (R_ss, R_nn), complex64 [len(slots), K, F, C, C]."""
+        idx = self._slot_list(slots)
+        if self._open[idx].any():
+            raise ValueError("slot %d is already open" % int(idx[self._open[idx]][0]))
+        K, C, F = self.K, self.C, self.F
+        if R0 is not None:
+            if not isinstance(R0, (tuple, list)) or len(R0) != 2:
+                raise ValueError("R0 must be the pair (R_ss, R_nn)")
+            for r in R0:
+                if not isinstance(r, torch.Tensor) or not r.is_cuda:
+                    raise TypeError("R0 must hold CUDA tensors (disco_b200 has no CPU path)")
+                if r.dtype != torch.complex64 or tuple(r.shape) != (len(idx), K, F, C, C) or r.device != self.device:
+                    raise ValueError("R0 matrices must be complex64 [%d, %d, %d, %d, %d] on %s"
+                                     % (len(idx), K, F, C, C, self.device))
+        if len(idx) == 0:
+            return
+        self._alloc()
+        i = torch.from_numpy(idx).to(self.device)
+        self._hist[:, i] = 0
+        self._carry[i] = 0
+        for buf in (self._Yblk, self._m1, self._m2, self._zblk):
+            if buf is not None:
+                buf[i] = 0
+        for w in range(2):
+            self._R1[w][i] = 0 if R0 is None else R0[w]
+            self._R2[w][i] = R0[w] if (R0 is not None and K == 1) else 0   # step 2 of a single node starts from R0
+        self._W1[i] = self._pass[0]
+        self._W2[i] = self._pass[1]
+        self._open[idx] = True
+        for a in (self._L, self._T, self._S, self._par, self._nclosed):
+            a[idx] = 0
+
+    def push(self, y, n, mask_fn):
+        """Append y[s, :, :, :n[s]] to slot s (y [S, K, C, n_max] float32 CUDA; n host ints, 0 <= n[s] <= n_max, and
+        0 for free slots); returns what became final (class doc)."""
+        if not isinstance(y, torch.Tensor):
+            raise TypeError("y must be a CUDA tensor (disco_b200 has no CPU path)")
+        if y.dim() != 4 or tuple(y.shape[:3]) != (self.S, self.K, self.C):
+            raise ValueError("y shape %s, expected (%d, %d, %d, n_max)" % (tuple(y.shape), self.S, self.K, self.C))
+        n_max = y.shape[-1]
+        n = np.asarray(n)
+        if n.dtype.kind not in "iu" or n.shape != (self.S,):
+            raise ValueError("n must hold one integer per slot")
+        n = n.astype(np.int64)
+        if np.any(n < 0) or np.any(n > n_max):
+            raise ValueError("every n[s] must lie in [0, %d]" % n_max)
+        if np.any(n[~self._open] > 0):
+            raise ValueError("samples pushed to free slot %d" % int(np.nonzero((n > 0) & ~self._open)[0][0]))
+        if not y.is_cuda:
+            raise TypeError("y must be a CUDA tensor (disco_b200 has no CPU path)")
+        if y.dtype != torch.float32:
+            raise TypeError("y must be float32, got %s" % y.dtype)
+        if y.device != self.device:
+            raise ValueError("y is on %s, the pool on %s" % (y.device, self.device))
+        H = self.n_fft // 2
+        L1 = self._L + n
+        T1 = np.where(self._open & (L1 > H), L1 // H, self._T)
+        S1 = np.where(self._open & (L1 > H), (L1 // H - 1) * H, self._S)
+        return self._run(y.contiguous(), n, L1, T1, S1, np.zeros(self.S, dtype=bool), mask_fn)
+
+    def close(self, slots, mask_fn):
+        """End the streams of `slots`: the last frame (reflected at the end), the final, partial block's statistics
+        and filters, and the remaining time samples up to samples_in.  The slots are free afterwards."""
+        idx = self._slot_list(slots)
+        if not self._open[idx].all():
+            raise ValueError("slot %d is not open" % int(idx[~self._open[idx]][0]))
+        H = self.n_fft // 2
+        if np.any(self._L[idx] <= H):
+            raise ValueError("a stream needs more than n_fft / 2 = %d samples (reflect padding)" % H)
+        final = np.zeros(self.S, dtype=bool)
+        final[idx] = True
+        T1, S1 = self._T.copy(), self._S.copy()
+        T1[idx] = 1 + self._L[idx] // H
+        S1[idx] = self._L[idx]
+        chunk = torch.empty((self.S, self.K, self.C, 0), dtype=torch.float32, device=self.device)
+        out = self._run(chunk, np.zeros(self.S, dtype=np.int64), self._L.copy(), T1, S1, final, mask_fn)
+        self._open[idx] = False
+        return out
+
+    # ---------------------------------------------------------------- internals
+    def _slot_list(self, slots):
+        idx = np.asarray(slots).reshape(-1)
+        if idx.size and idx.dtype.kind not in "iu":
+            raise ValueError("slots must be integers")
+        idx = idx.astype(np.int64)
+        if np.any(idx < 0) or np.any(idx >= self.S):
+            raise ValueError("slots must lie in 0..%d" % (self.S - 1))
+        if len(np.unique(idx)) != len(idx):
+            raise ValueError("a slot is listed twice")
+        return idx
+
+    def _run(self, chunk, n, L1, T1, S1, final, mask_fn):
+        touched = (n > 0) | (T1 > self._T) | final
+        try:
+            return self._advance(chunk, n, L1, T1, S1, final, mask_fn)
+        except BaseException:
+            self._open[touched] = False
+            raise
+
+    def _masks(self, masks, f):
+        if not isinstance(masks, (tuple, list)) or len(masks) != 2:
+            raise ValueError("mask_fn must return the pair (mask_z, mask_w)")
+        mz, mw = masks
+        mw = mz if mw is None else mw
+        want = (self.S, self.K, f, self.F)
+        for m, name in ((mz, "mask_z"), (mw, "mask_w")):
+            if not isinstance(m, torch.Tensor):
+                raise ValueError("%s must be a tensor %s" % (name, want))
+            if tuple(m.shape) != want:
+                raise ValueError("%s shape %s, expected %s" % (name, tuple(m.shape), want))
+            if m.dtype != torch.float32 or m.device != self.device:
+                raise ValueError("%s must be float32 on %s" % (name, self.device))
+        return mz, mw
+
+    def _close_blocks(self, cl, nb, ci):
+        """Statistics and filters of the open block of the slots `cl` (ci: the same indices on the device) once the
+        masks of its nb[s] frames are in (nb < block: the final, partial block, whose recursion step is lambda^nb)."""
+        P, lam, n_fft = self.block, self.lambda_cor, self.n_fft
+        Yb, m1, m2 = self._Yblk[ci], self._m1[ci], self._m2[ci]
+        zb = self._zblk[ci] if self.K > 1 else None
+        R1 = (self._R1[0][ci], self._R1[1][ci])
+        R2 = (self._R2[0][ci], self._R2[1][ci])
+        Rs1, Rn1 = ops.scm_recursive(Yb, m1, None, lam, P, 2, R1, n_fft, frames=nb)
+        Rs2, Rn2 = ops.scm_recursive(Yb, m2, zb, lam, P, 2, R2, n_fft, frames=nb)
+        W1 = ops.mwf_solve(Rs1, Rn1, self.mu, "gevd", self.rank)[0][:, :, 0]
+        W2 = ops.mwf_solve(Rs2, Rn2, self.mu, "gevd", self.rank)[0][:, :, 0]
+        for R, new in ((self._R1, (Rs1, Rn1)), (self._R2, (Rs2, Rn2))):
+            R[0][ci] = new[0][:, :, 0]
+            R[1][ci] = new[1][:, :, 0]
+        pos = torch.from_numpy(self._nclosed[cl] % (self.lag + 1)).to(self.device)
+        self._W1[ci, pos] = W1
+        self._W2[ci, pos] = W2
+        self._nclosed[cl] += 1
+
+    def _advance(self, chunk, n, L1, T1, S1, final, mask_fn):
+        S, K, F, P, lag, n_fft, ref, dev = (self.S, self.K, self.F, self.block, self.lag, self.n_fft, self.ref_mic,
+                                            self.device)
+        T0, S0 = self._T.copy(), self._S.copy()
+        frames, samples = T1 - T0, S1 - S0
+        starts, runs = pool_rounds(T0, T1, P)
+        c64 = dict(dtype=torch.complex64, device=dev)
+        f_call = int(frames.max())
+        out = [torch.zeros((S, K, f_call, F), **c64) for _ in range(3)]        # z_y, zn, yf
+        yf_time = torch.zeros((S, K, int(samples.max())), dtype=torch.float32, device=dev)
+        write = n > 0
+        stft_rec = np.zeros((S, len(ops.STFT_SLOT_FIELDS)), dtype=np.int64)
+        stft_rec[:, 0], stft_rec[:, 1], stft_rec[:, 5], stft_rec[:, 6] = L1, n, final, self._par
+        istft_rec = np.zeros((S, len(ops.ISTFT_SLOT_FIELDS)), dtype=np.int64)
+        istft_rec[:, 2], istft_rec[:, 4] = L1, S0
+        if len(runs) == 0 and write.any():       # no frame completes: only the history moves
+            stft_rec[:, 2], stft_rec[:, 7] = T0, write
+            ops.stream_stft_slots(self._hist, chunk, stft_rec, 0, n_fft)
+        for r in range(len(runs)):
+            t0, nr = starts[r], runs[r]
+            act = np.nonzero(nr)[0]
+            fr, f = nr[act], int(nr.max())
+            blk = np.where(nr > 0, t0 % P, 0)
+            stft_rec[:, 2], stft_rec[:, 3], stft_rec[:, 4], stft_rec[:, 7] = t0, nr, blk, write if r == 0 else 0
+            Y = ops.stream_stft_slots(self._hist, chunk, stft_rec, f, n_fft, Y_blk=self._Yblk)
+            # one host -> device copy per round: active slots, ring positions, and the (slot, frame) pairs of the run
+            s_idx = np.repeat(act, fr)
+            a_idx = np.repeat(np.arange(len(act)), fr)
+            i_idx = np.arange(len(s_idx)) - np.repeat(np.cumsum(fr) - fr, fr)
+            pos = (t0[act] // P - lag) % (lag + 1)
+            host = np.concatenate([act, pos, s_idx, a_idx, i_idx, blk[s_idx] + i_idx, (t0 - T0)[s_idx] + i_idx])
+            d = torch.from_numpy(host).to(dev)
+            na, nf = len(act), len(s_idx)
+            ai, pi = d[:na], d[na:2 * na]
+            si, aj, ii, bi, oi = (d[2 * na + k * nf:2 * na + (k + 1) * nf] for k in range(5))
+            every = na == S
+            Ya = Y if every else Y[ai]
+            # step 1 and step 2 with the filter in force, W_(j - lag) (the pass-through stand-in before the first)
+            z, zn = ops.filter_sum_blocks(self._W1[ai, pi].unsqueeze(2), Ya, None, P, 0, True, ref, n_fft, frames=fr)
+            yf, _ = ops.filter_sum_blocks(self._W2[ai, pi].unsqueeze(2), Ya, z if K > 1 else None, P, 0, True, ref,
+                                          n_fft, frames=fr)
+            if every:
+                zf, znf, yff = z, zn, yf
+            else:
+                zf, znf, yff = (torch.zeros((S, K, f, F), **c64) for _ in range(3))
+                zf[ai], znf[ai], yff[ai] = z, zn, yf
+            mz, mw = self._masks(mask_fn(t0.copy(), nr.copy(), Y, zf, znf), f)
+            self._m1[si, :, bi] = mz[si, :, ii]
+            self._m2[si, :, bi] = mw[si, :, ii]
+            if K > 1:
+                self._zblk[si, :, bi] = z[aj, :, ii]
+            for o, v in zip(out, (z, zn, yf)):
+                o[si, :, oi] = v[aj, :, ii]
+            ends = t0 + nr
+            closing = (nr > 0) & ((blk + nr == P) | (final & (ends == T1)))
+            if closing.any():
+                cl = np.nonzero(closing)[0]
+                self._close_blocks(cl, (blk + nr)[cl], ai if every and len(cl) == S else torch.from_numpy(cl).to(dev))
+            istft_rec[:, 0], istft_rec[:, 1], istft_rec[:, 3] = t0, nr, final & (nr > 0) & (ends == T1)
+            ops.stream_istft_slots(yff, self._carry, istft_rec, yf_time, n_fft)
+        self._par = np.where(write, 1 - self._par, self._par)
+        self._L, self._T, self._S = L1.copy(), T1.copy(), S1.copy()
+        return {"t0": T0, "frames": frames, "s0": S0, "samples": samples, "z_y": out[0], "zn": out[1], "yf": out[2],
+                "yf_time": yf_time}

@@ -303,6 +303,29 @@ DISCO_API int disco_stream_stft(const float* hist, const float* chunk, float* hi
                                 int final_call, int n_fft, void* stream);
 DISCO_API int disco_stream_istft(const void* Y, float* carry, float* x, int n_sig, int t0, int n_fr, int length,
                                  int final_call, int x_first, int x_stride, int n_fft, void* stream);
+/* The same two calls on a pool of n_slot independent streams of n_sig signals each (disco_b200/stream.py,
+ * OnlineTangoPool).  Slot s owns signals [s n_sig, (s + 1) n_sig); signals 2p and 2p + 1 of ONE slot share a transform
+ * and an odd last signal runs alone, so every slot's outputs are bit-identical to the single-stream call on that slot
+ * alone (n_sig signals), whatever the other slots hold.  Each slot has a record of ints; `slots` is the device copy the
+ * kernels read and `slots_host` the same values in host memory, checked before anything is launched with the
+ * single-stream checks applied per slot (DISCO_ERR_INVALID).
+ * disco_stream_stft_slots, record [n_slot][8] = {length, n_new, t0, n_fr, blk_slot, final, hist_sel, hist_write}:
+ *   hist  [2][n_slot][n_sig][n_fft] float32: buffer hist_sel of slot s holds its samples [L0 - n_fft, L0), L0 =
+ *         length - n_new; with hist_write = 1 its samples [length - n_fft, length) are written to the other buffer
+ *   chunk [n_slot][n_sig][n_max] float32: samples [L0, length) at the start of each row (0 <= n_new <= n_max)
+ *   Y     [n_slot][n_sig][f_max][F] complex64 out: frames t0 .. t0 + n_fr - 1 (n_fr <= f_max) at rows 0 .. n_fr - 1
+ *   Y_blk (may be NULL) [n_slot][n_sig][blk_frames][F]: the same frames at rows blk_slot .. blk_slot + n_fr - 1
+ *   A slot with n_fr = 0 and hist_write = 0 is not touched.
+ * disco_stream_istft_slots, record [n_slot][5] = {t0, n_fr, length, final, x_first}:
+ *   Y     [n_slot][n_sig][f_max][F]: frames t0 .. t0 + n_fr - 1 of slot s at rows 0 .. n_fr - 1
+ *   carry [n_slot][n_sig][n_fft / 2], updated in place
+ *   x     [n_slot][n_sig][s_max]: sample i of slot s at i - x_first
+ *   A slot with n_fr = 0 that is not final is not touched. */
+DISCO_API int disco_stream_stft_slots(float* hist, const float* chunk, void* Y, void* Y_blk, const int* slots,
+                                      const int* slots_host, int n_slot, int n_sig, int n_max, int f_max,
+                                      int blk_frames, int n_fft, void* stream);
+DISCO_API int disco_stream_istft_slots(const void* Y, float* carry, float* x, const int* slots, const int* slots_host,
+                                       int n_slot, int n_sig, int f_max, int s_max, int n_fft, void* stream);
 
 /* ---- IIR filter bank + band statistics -------------------------------------------------------------
  * Replaces, for every band i of a filter bank, `y = scipy.signal.lfilter(b[i], a[i], x)` followed by the

@@ -96,3 +96,22 @@ for (B, K, C, L, n_fft, block) in ((3, 1, 4, 6000, 512, 8), (3, 8, 2, 5000, 256,
     td = post.to_time(out, L, n_fft=n_fft, names=("yf", "z_y"), layout="TF", lengths=lengths)
     torch.cuda.synchronize()
     print("ok online lengths", B, K, C, n_fft, block, float(td["yf"].abs().mean()))
+# pool of independent streams: per-slot STFT / iSTFT (odd K C: a lone last signal), slots opening, idling, closing and
+# reopening, block closes on a subset of the slots
+from disco_b200.stream import OnlineTangoPool
+for (S, K, C, n_fft, block) in ((3, 1, 3, 256, 4), (2, 2, 3, 1024, 2), (2, 8, 2, 512, 3)):
+    pool = OnlineTangoPool(S, K, C, n_fft=n_fft, block=block, device=dev)
+    fn = lambda t0, n_fr, Y, z, zn: (torch.rand(z.shape, device=dev), None)
+    H = n_fft // 2
+    pool.open([0])
+    pool.push(torch.randn(S, K, C, 3 * H + 5, device=dev), np.array([3 * H + 5] + [0] * (S - 1)), fn)
+    pool.open(list(range(1, S)))
+    for n in ((1, H - 1), (5 * H, 0), (0, 2 * H + 1)):
+        nn = np.array([n[s % 2] for s in range(S)])
+        pool.push(torch.randn(S, K, C, max(int(nn.max()), 1), device=dev), nn, fn)
+    pool.close([0], fn)
+    pool.open([0])
+    pool.push(torch.randn(S, K, C, 4 * H, device=dev), np.full(S, 4 * H), fn)
+    out = pool.close(list(range(S)), fn)
+    torch.cuda.synchronize()
+    print("ok pool", S, K, C, n_fft, pool.frames_out.tolist(), float(out["yf_time"].abs().mean()))
