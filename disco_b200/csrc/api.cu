@@ -667,46 +667,76 @@ int disco_filter_sum_blocks_lengths(const void* W, int conj_w, const void* Y, co
                                     n_sel, frames, frames_host, stream);
 }
 
+// A stream STFT record against the buffers it addresses: chunk rows of n_max samples, f_max frame rows of Y, and
+// (Y_blk) blk_frames rows of the block buffer
+static int check_stft_record(const StftSlot& r, int n_fft, int n_max, int f_max, int blk_frames, const void* chunk,
+                             const void* Y, const void* Y_blk) {
+    if (r.n_new < 0 || r.n_new > n_max || r.length < r.n_new || r.t0 < 0 || r.n_fr < 0 || r.n_fr > f_max ||
+        (r.hist_sel != 0 && r.hist_sel != 1))
+        return fail(DISCO_ERR_INVALID, "bad sizes");
+    if ((r.n_new > 0 && !chunk) || (r.n_fr > 0 && !Y) || (r.final_call && r.n_new > 0))
+        return fail(DISCO_ERR_INVALID, "null pointer (or a chunk on the final call)");
+    if (r.n_fr > 0) {
+        // every sample the frames read has arrived (the last frame is reflected at the end on the final call), and
+        // the first one lies within the carried history
+        const int H = n_fft / 2, L0 = r.length - r.n_new, t1 = r.t0 + r.n_fr - 1;
+        const bool arrived = r.length > H && (r.final_call ? t1 <= r.length / H : (t1 == 0 || (t1 + 1) * H <= r.length));
+        if (!arrived || (r.t0 >= 1 && (r.t0 - 1) * H < L0 - n_fft))
+            return fail(DISCO_ERR_INVALID, "frames not complete, or older than the carried history");
+        if (Y_blk && (r.blk_slot < 0 || r.blk_slot + r.n_fr > blk_frames))
+            return fail(DISCO_ERR_INVALID, "frames outside the block buffer");
+    }
+    return 0;
+}
+
+// A stream iSTFT record against the buffers it addresses: f_max frame rows of Y and rows of s_max samples of x
+static int check_istft_record(const IstftSlot& r, int n_fft, int f_max, int s_max, const void* Y, const float* x) {
+    if (r.t0 < 0 || r.n_fr < 0 || r.n_fr > f_max || r.x_first < 0 || (r.length < 1 && (r.n_fr > 0 || r.final_call)))
+        return fail(DISCO_ERR_INVALID, "bad sizes");
+    if (r.n_fr > 0 && !Y) return fail(DISCO_ERR_INVALID, "null pointer");
+    if (r.n_fr <= 0 && !r.final_call) return 0;   // not run
+    // samples written: the hop blocks max(t0, 1) .. t0 + n_fr - 1, and on the final call the rest up to length
+    const int H = n_fft / 2;
+    const int lo = (r.t0 > 0 ? r.t0 - 1 : 0) * H;
+    int hi = r.final_call ? r.length : (r.t0 + r.n_fr - 1) * H;
+    if (hi > r.length) hi = r.length;
+    if (hi > lo) {
+        if (!x) return fail(DISCO_ERR_INVALID, "null pointer");
+        if (lo < r.x_first || hi > r.x_first + s_max) return fail(DISCO_ERR_INVALID, "output samples outside x");
+    }
+    return 0;
+}
+
+// disco_stream_stft is one slot whose record is passed by value: the history is read from `hist` (hist_sel = 0) and
+// written to hist_out when there is one
 int disco_stream_stft(const float* hist, const float* chunk, float* hist_out, void* Y, void* Y_blk, int n_sig,
                       int n_new, int length, int t0, int n_fr, int blk_frames, int blk_slot, int final_call, int n_fft,
                       void* stream) {
     if (!valid_nfft(n_fft)) return fail(DISCO_ERR_INVALID, "n_fft must be 256, 512 or 1024");
     if (n_sig <= 0 || (n_sig + 1) / 2 > kMaxGridYZ) return fail(DISCO_ERR_INVALID, "n_sig must be in 1..131070");
-    if (n_new < 0 || length < n_new || t0 < 0 || n_fr < 0) return fail(DISCO_ERR_INVALID, "bad sizes");
-    if (!hist || (n_new > 0 && !chunk) || (n_fr > 0 && !Y) || (final_call && n_new > 0))
-        return fail(DISCO_ERR_INVALID, "null pointer (or a chunk on the final call)");
-    const int H = n_fft / 2, L0 = length - n_new;
-    if (n_fr > 0) {
-        // every sample the frames read has arrived (the last frame is reflected at the end on the final call), and
-        // the first one lies within the carried history
-        const int t1 = t0 + n_fr - 1;
-        const bool arrived = length > H && (final_call ? t1 <= length / H : (t1 == 0 || (t1 + 1) * H <= length));
-        if (!arrived || (t0 >= 1 && (t0 - 1) * H < L0 - n_fft))
-            return fail(DISCO_ERR_INVALID, "frames not complete, or older than the carried history");
-        if (Y_blk && (blk_slot < 0 || blk_slot + n_fr > blk_frames))
-            return fail(DISCO_ERR_INVALID, "frames outside the block buffer");
-    }
+    if (!hist) return fail(DISCO_ERR_INVALID, "null pointer");
+    const StftSlot r = {length, n_new, t0, n_fr, blk_slot, final_call ? 1 : 0, 0, hist_out ? 1 : 0};
+    int rc = check_stft_record(r, n_fft, n_new, n_fr, blk_frames, chunk, Y, Y_blk);
+    if (rc) return rc;
     Tables tb;
-    int rc = get_tables(n_fft, &tb);
+    rc = get_tables(n_fft, &tb);
     if (rc) return rc;
     StreamStftArgs a;
     memset(&a, 0, sizeof(a));
-    a.hist = hist;
+    a.hist[0] = const_cast<float*>(hist);   // hist_sel = 0: read only
+    a.hist[1] = hist_out;
     a.chunk = chunk;
-    a.hist_out = hist_out;
     a.Y = (float2*)Y;
     a.Y_blk = (float2*)Y_blk;
     a.twiddle = tb.twiddle;
     a.window = tb.win_half;
+    a.one = r;
+    a.n_slot = 1;
     a.n_sig = n_sig;
-    a.n_new = n_new;
-    a.length = length;
-    a.t0 = t0;
-    a.n_fr = n_fr;
+    a.n_max = n_new;
+    a.f_max = n_fr;
     a.blk_frames = blk_frames;
-    a.blk_slot = blk_slot;
-    a.final_call = final_call ? 1 : 0;
-    CU(launch_stream_stft(a, n_fft, (cudaStream_t)stream), "stream_stft launch");
+    CU(launch_stream_stft_slots(a, n_fft, (cudaStream_t)stream), "stream_stft launch");
     return 0;
 }
 
@@ -714,19 +744,13 @@ int disco_stream_istft(const void* Y, float* carry, float* x, int n_sig, int t0,
                        int x_first, int x_stride, int n_fft, void* stream) {
     if (!valid_nfft(n_fft)) return fail(DISCO_ERR_INVALID, "n_fft must be 256, 512 or 1024");
     if (n_sig <= 0 || (n_sig + 1) / 2 > kMaxGridYZ) return fail(DISCO_ERR_INVALID, "n_sig must be in 1..131070");
-    if (t0 < 0 || n_fr < 0 || length < 1 || x_first < 0 || x_stride < 0) return fail(DISCO_ERR_INVALID, "bad sizes");
-    if (!carry || (n_fr > 0 && !Y)) return fail(DISCO_ERR_INVALID, "null pointer");
-    const int H = n_fft / 2;
-    // samples written: the hop blocks max(t0, 1) .. t0 + n_fr - 1, and on the final call the rest up to length
-    const int lo = (t0 > 0 ? t0 - 1 : 0) * H;
-    int hi = final_call ? length : (t0 + n_fr - 1) * H;
-    if (hi > length) hi = length;
-    if (hi > lo) {
-        if (!x) return fail(DISCO_ERR_INVALID, "null pointer");
-        if (lo < x_first || hi > x_first + x_stride) return fail(DISCO_ERR_INVALID, "output samples outside x");
-    }
+    if (length < 1 || x_stride < 0) return fail(DISCO_ERR_INVALID, "bad sizes");
+    if (!carry) return fail(DISCO_ERR_INVALID, "null pointer");
+    const IstftSlot r = {t0, n_fr, length, final_call ? 1 : 0, x_first};
+    int rc = check_istft_record(r, n_fft, n_fr, x_stride, Y, x);
+    if (rc) return rc;
     Tables tb;
-    int rc = get_tables(n_fft, &tb);
+    rc = get_tables(n_fft, &tb);
     if (rc) return rc;
     IstftArgs a;
     memset(&a, 0, sizeof(a));
@@ -736,19 +760,13 @@ int disco_stream_istft(const void* Y, float* carry, float* x, int n_sig, int t0,
     a.twiddle = tb.twiddle;
     a.window = tb.win;
     a.n_sig = n_sig;
-    a.L = length;
     a.y_frames = n_fr;
-    a.y_t0 = t0;
     a.ld = x_stride;
-    a.x_first = x_first;
-    a.j_begin = t0;
-    a.j_end = t0 + n_fr;
-    a.tail = final_call ? 1 : 0;
-    CU(launch_istft(a, n_fft, (cudaStream_t)stream), "stream_istft launch");
+    CU(launch_stream_istft_slots(a, nullptr, r, 1, n_fft, (cudaStream_t)stream), "stream_istft launch");
     return 0;
 }
 
-// disco_stream_stft_slots: the per-slot versions of disco_stream_stft's checks, on the host copy of the records
+// disco_stream_stft_slots: disco_stream_stft's record check per slot, on the host copy of the records
 int disco_stream_stft_slots(float* hist, const float* chunk, void* Y, void* Y_blk, const int* slots,
                             const int* slots_host, int n_slot, int n_sig, int n_max, int f_max, int blk_frames,
                             int n_fft, void* stream) {
@@ -757,47 +775,34 @@ int disco_stream_stft_slots(float* hist, const float* chunk, void* Y, void* Y_bl
     if (n_sig <= 0 || (n_sig + 1) / 2 > kMaxGridYZ) return fail(DISCO_ERR_INVALID, "n_sig must be in 1..131070");
     if (n_max < 0 || f_max < 0 || blk_frames < 0) return fail(DISCO_ERR_INVALID, "bad sizes");
     if (!slots_host || !slots || !hist) return fail(DISCO_ERR_INVALID, "null pointer");
-    const int H = n_fft / 2;
+    const StftSlot* recs = (const StftSlot*)slots_host;
     for (int s = 0; s < n_slot; ++s) {
-        const int* r = slots_host + (size_t)s * kStftSlotFields;
-        const int length = r[0], n_new = r[1], t0 = r[2], n_fr = r[3], blk_slot = r[4], final_call = r[5];
-        const int sel = r[6];
-        if (n_new < 0 || n_new > n_max || length < n_new || t0 < 0 || n_fr < 0 || n_fr > f_max || (sel != 0 && sel != 1))
-            return fail(DISCO_ERR_INVALID, "bad sizes in a slot record");
-        if ((n_new > 0 && !chunk) || (n_fr > 0 && !Y) || (final_call && n_new > 0))
-            return fail(DISCO_ERR_INVALID, "null pointer (or a chunk on a slot's final call)");
-        const int L0 = length - n_new;
-        if (n_fr > 0) {
-            const int t1 = t0 + n_fr - 1;
-            const bool arrived = length > H && (final_call ? t1 <= length / H : (t1 == 0 || (t1 + 1) * H <= length));
-            if (!arrived || (t0 >= 1 && (t0 - 1) * H < L0 - n_fft))
-                return fail(DISCO_ERR_INVALID, "a slot's frames are not complete, or older than its carried history");
-            if (Y_blk && (blk_slot < 0 || blk_slot + n_fr > blk_frames))
-                return fail(DISCO_ERR_INVALID, "a slot's frames lie outside the block buffer");
-        }
+        const int rc = check_stft_record(recs[s], n_fft, n_max, f_max, blk_frames, chunk, Y, Y_blk);
+        if (rc) return rc;
     }
     Tables tb;
     int rc = get_tables(n_fft, &tb);
     if (rc) return rc;
-    StreamStftSlotsArgs a;
+    StreamStftArgs a;
     memset(&a, 0, sizeof(a));
-    a.hist = hist;
+    a.hist[0] = hist;
+    a.hist[1] = hist + (size_t)n_slot * n_sig * n_fft;
     a.chunk = chunk;
     a.Y = (float2*)Y;
     a.Y_blk = (float2*)Y_blk;
     a.twiddle = tb.twiddle;
     a.window = tb.win_half;
-    a.n_sig = n_sig;
-    a.blk_frames = blk_frames;
-    a.slots = slots;
+    a.slots = (const StftSlot*)slots;
     a.n_slot = n_slot;
+    a.n_sig = n_sig;
     a.n_max = n_max;
     a.f_max = f_max;
+    a.blk_frames = blk_frames;
     CU(launch_stream_stft_slots(a, n_fft, (cudaStream_t)stream), "stream_stft_slots launch");
     return 0;
 }
 
-// disco_stream_istft_slots: the per-slot versions of disco_stream_istft's checks, on the host copy of the records
+// disco_stream_istft_slots: disco_stream_istft's record check per slot, on the host copy of the records
 int disco_stream_istft_slots(const void* Y, float* carry, float* x, const int* slots, const int* slots_host,
                              int n_slot, int n_sig, int f_max, int s_max, int n_fft, void* stream) {
     if (!valid_nfft(n_fft)) return fail(DISCO_ERR_INVALID, "n_fft must be 256, 512 or 1024");
@@ -805,21 +810,10 @@ int disco_stream_istft_slots(const void* Y, float* carry, float* x, const int* s
     if (n_sig <= 0 || (n_sig + 1) / 2 > kMaxGridYZ) return fail(DISCO_ERR_INVALID, "n_sig must be in 1..131070");
     if (f_max < 0 || s_max < 0) return fail(DISCO_ERR_INVALID, "bad sizes");
     if (!slots_host || !slots || !carry) return fail(DISCO_ERR_INVALID, "null pointer");
-    const int H = n_fft / 2;
+    const IstftSlot* recs = (const IstftSlot*)slots_host;
     for (int s = 0; s < n_slot; ++s) {
-        const int* r = slots_host + (size_t)s * kIstftSlotFields;
-        const int t0 = r[0], n_fr = r[1], length = r[2], final_call = r[3], x_first = r[4];
-        if (t0 < 0 || n_fr < 0 || n_fr > f_max || x_first < 0 || (length < 1 && (n_fr > 0 || final_call)))
-            return fail(DISCO_ERR_INVALID, "bad sizes in a slot record");
-        if (n_fr > 0 && !Y) return fail(DISCO_ERR_INVALID, "null pointer");
-        if (n_fr <= 0 && !final_call) continue;   // the slot is not run
-        const int lo = (t0 > 0 ? t0 - 1 : 0) * H;
-        int hi = final_call ? length : (t0 + n_fr - 1) * H;
-        if (hi > length) hi = length;
-        if (hi > lo) {
-            if (!x) return fail(DISCO_ERR_INVALID, "null pointer");
-            if (lo < x_first || hi > x_first + s_max) return fail(DISCO_ERR_INVALID, "a slot's output samples lie outside x");
-        }
+        const int rc = check_istft_record(recs[s], n_fft, f_max, s_max, Y, x);
+        if (rc) return rc;
     }
     Tables tb;
     int rc = get_tables(n_fft, &tb);
@@ -834,7 +828,9 @@ int disco_stream_istft_slots(const void* Y, float* carry, float* x, const int* s
     a.n_sig = n_sig;
     a.y_frames = f_max;
     a.ld = s_max;
-    CU(launch_stream_istft_slots(a, slots, n_slot, n_fft, (cudaStream_t)stream), "stream_istft_slots launch");
+    const IstftSlot none = {};
+    CU(launch_stream_istft_slots(a, (const IstftSlot*)slots, none, n_slot, n_fft, (cudaStream_t)stream),
+       "stream_istft_slots launch");
     return 0;
 }
 

@@ -1,6 +1,6 @@
 // Inverse STFT with overlap-add and window-sum-square normalisation, batched: disco_istft over whole signals and
-// disco_stream_istft over the new frames of a stream run one kernel body (istft_body), so a stream's time samples
-// equal those of the whole-signal call value for value.
+// disco_stream_istft / disco_stream_istft_slots over the new frames of a stream run one kernel body (istft_body), so a
+// stream's time samples equal those of the whole-signal call value for value.
 //
 // Replaces lb.core.istft(S, hop_length=N/2, win_length=N, center=True, length=L)
 // (reference tango.py:528-539, math_utils.py:143-152; librosa <= 0.9 semantics, SURVEY App. A.2):
@@ -176,10 +176,6 @@ template <int N>
 __global__ void __launch_bounds__(IGeom<N>::THREADS) istft_kernel(IstftArgs p) {
     istft_body<N, false>(p);
 }
-template <int N>
-__global__ void __launch_bounds__(IGeom<N>::THREADS) stream_istft_kernel(IstftArgs p) {
-    istft_body<N, true>(p);
-}
 
 // Whole signals of their own lengths (disco_istft_lengths, launched from lengths.cu): signal s is the iSTFT of its
 // frames [0, min(j_end, 1 + lengths[s] / H)) cut to lengths[s] samples, exactly as disco_istft runs it on those frames
@@ -218,46 +214,49 @@ __global__ void __launch_bounds__(IGeom<N>::THREADS) istft_lengths_kernel(IstftA
     }
 }
 
-// A pool of independent streams (disco_stream_istft_slots): grid (1, pairs of a slot, slots).  Slot blockIdx.z runs the
-// stream body on its own rows with its record {t0, n_fr, length, final, x_first}, as disco_stream_istft runs it on
-// that slot alone.
+// A stream: grid (1, signal pairs of a slot, slots).  Slot blockIdx.z runs the stream body on its own rows with its
+// record {t0, n_fr, length, final, x_first}: from `slots` (a pool) or, with slots = null, `one` (a lockstep stream).
 template <int N>
-__global__ void __launch_bounds__(IGeom<N>::THREADS) stream_istft_slots_kernel(IstftArgs p, const int* slots) {
+__global__ void __launch_bounds__(IGeom<N>::THREADS) stream_istft_kernel(IstftArgs p, const IstftSlot* slots,
+                                                                         IstftSlot one) {
     constexpr int H = IGeom<N>::H, F = IGeom<N>::F;
-    const int* r = slots + (size_t)blockIdx.z * kIstftSlotFields;
-    const int t0 = r[0], n_fr = r[1];
-    if (n_fr <= 0 && !r[3]) return;   // CTA-uniform: no frames, not the end of the stream
+    IstftSlot r = one;
+    if (slots) r = slots[blockIdx.z];
+    if (r.n_fr <= 0 && !r.final_call) return;   // CTA-uniform: no frames, not the end of the stream
     IstftArgs q = p;
     const size_t row0 = (size_t)blockIdx.z * p.n_sig;
     q.Y = p.Y + row0 * p.y_frames * F;
     q.x = p.x ? p.x + row0 * p.ld : nullptr;
     q.carry = p.carry + row0 * H;
-    q.L = r[2];
-    q.y_t0 = t0;
-    q.j_begin = t0;
-    q.j_end = t0 + n_fr;
-    q.fpc = n_fr;
-    q.tail = r[3];
-    q.x_first = r[4];
+    q.L = r.length;
+    q.y_t0 = r.t0;
+    q.j_begin = r.t0;
+    q.j_end = r.t0 + r.n_fr;
+    q.fpc = r.n_fr;
+    q.tail = r.final_call;
+    q.x_first = r.x_first;
     istft_body<N, true>(q);
 }
 
 template <int N>
-static cudaError_t launch_slots_n(const IstftArgs& a, const int* slots, int n_slot, cudaStream_t st) {
+static cudaError_t launch_slots_n(const IstftArgs& a, const IstftSlot* slots, const IstftSlot& one, int n_slot,
+                                   cudaStream_t st) {
     using G = IGeom<N>;
-    cudaError_t e = cudaFuncSetAttribute(stream_istft_slots_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e = cudaFuncSetAttribute(stream_istft_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          (int)G::SMEM);
     if (e != cudaSuccess) return e;
-    stream_istft_slots_kernel<N><<<dim3(1, (a.n_sig + 1) / 2, n_slot), G::THREADS, G::SMEM, st>>>(a, slots);
+    stream_istft_kernel<N><<<dim3(1, (a.n_sig + 1) / 2, n_slot), G::THREADS, G::SMEM, st>>>(a, slots, one);
     return cudaGetLastError();
 }
 
-cudaError_t launch_stream_istft_slots(const IstftArgs& a, const int* slots, int n_slot, int n_fft, cudaStream_t st) {
-    if (a.n_sig <= 0 || n_slot <= 0) return cudaSuccess;
+// n_slot slots; a lockstep stream is one slot whose record is `one`
+cudaError_t launch_stream_istft_slots(const IstftArgs& a, const IstftSlot* slots, const IstftSlot& one, int n_slot,
+                                      int n_fft, cudaStream_t st) {
+    if (a.n_sig <= 0 || n_slot <= 0 || (!slots && one.n_fr <= 0 && !one.final_call)) return cudaSuccess;
     switch (n_fft) {
-        case 256: return launch_slots_n<256>(a, slots, n_slot, st);
-        case 512: return launch_slots_n<512>(a, slots, n_slot, st);
-        case 1024: return launch_slots_n<1024>(a, slots, n_slot, st);
+        case 256: return launch_slots_n<256>(a, slots, one, n_slot, st);
+        case 512: return launch_slots_n<512>(a, slots, one, n_slot, st);
+        case 1024: return launch_slots_n<1024>(a, slots, one, n_slot, st);
         default: return cudaErrorInvalidValue;
     }
 }
@@ -277,26 +276,18 @@ static cudaError_t launch_n(IstftArgs a, cudaStream_t st) {
     using G = IGeom<N>;
     const int H = G::H;
     const int pairs = (a.n_sig + 1) / 2;
+    // the blocks past the last sample are not computed; chunks of fpc blocks
+    a.j_end = min(a.j_end, (a.L + N + H - 1) / H);
+    const int T_eff = a.j_end - a.j_begin;
+    if (T_eff < 1) return cudaErrorInvalidValue;
     int chunks = 1;
-    if (!a.carry) {   // whole signals: the blocks past the last sample are not computed; chunks of fpc blocks
-        a.j_end = min(a.j_end, (a.L + N + H - 1) / H);
-        const int T_eff = a.j_end - a.j_begin;
-        if (T_eff < 1) return cudaErrorInvalidValue;
-        while (pairs * chunks < sm_count() * 2 && (T_eff + chunks - 1) / chunks > 4 * G::ITEMS) chunks *= 2;
-        a.fpc = ((T_eff + chunks - 1) / chunks + G::ITEMS - 1) / G::ITEMS * G::ITEMS;
-        chunks = (T_eff + a.fpc - 1) / a.fpc;
-    } else {          // a stream: one CTA per pair runs all the new blocks
-        a.fpc = a.j_end - a.j_begin;
-    }
-    auto kern = a.carry ? stream_istft_kernel<N> : istft_kernel<N>;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G::SMEM);
+    while (pairs * chunks < sm_count() * 2 && (T_eff + chunks - 1) / chunks > 4 * G::ITEMS) chunks *= 2;
+    a.fpc = ((T_eff + chunks - 1) / chunks + G::ITEMS - 1) / G::ITEMS * G::ITEMS;
+    chunks = (T_eff + a.fpc - 1) / a.fpc;
+    cudaError_t e = cudaFuncSetAttribute(istft_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G::SMEM);
     if (e != cudaSuccess) return e;
-    if (a.carry) {    // the stream's signal count is bounded by its ABI (one launch of at most kMaxGridYZ pairs)
-        kern<<<dim3(chunks, pairs), G::THREADS, G::SMEM, st>>>(a);
-        return cudaGetLastError();
-    }
-    // pairs sit in grid.y: whole signals run in consecutive launches of at most kMaxGridYZ pairs, each starting at an
-    // even signal (a pair keeps its partner) with Y and x advanced to it (whole-signal rows are contiguous per signal)
+    // pairs sit in grid.y: consecutive launches of at most kMaxGridYZ pairs, each starting at an even signal (a pair
+    // keeps its partner) with Y and x advanced to it (whole-signal rows are contiguous per signal)
     const int n_sig = a.n_sig, F = N / 2 + 1;
     for (int p0 = 0; p0 < pairs; p0 += kMaxGridYZ) {
         IstftArgs b = a;
@@ -304,15 +295,16 @@ static cudaError_t launch_n(IstftArgs a, cudaStream_t st) {
         b.Y = a.Y + (size_t)s0 * a.y_frames * F;
         b.x = a.x + (size_t)s0 * a.ld;
         b.n_sig = min(n_sig - s0, 2 * kMaxGridYZ);
-        kern<<<dim3(chunks, (b.n_sig + 1) / 2), G::THREADS, G::SMEM, st>>>(b);
+        istft_kernel<N><<<dim3(chunks, (b.n_sig + 1) / 2), G::THREADS, G::SMEM, st>>>(b);
         e = cudaGetLastError();
         if (e != cudaSuccess) return e;
     }
     return cudaSuccess;
 }
 
+// Whole signals (a.carry = null, a.tail = 1)
 cudaError_t launch_istft(const IstftArgs& a, int n_fft, cudaStream_t st) {
-    if (a.n_sig <= 0 || (a.j_end <= a.j_begin && !a.tail)) return cudaSuccess;
+    if (a.n_sig <= 0) return cudaSuccess;
     switch (n_fft) {
         case 256: return launch_n<256>(a, st);
         case 512: return launch_n<512>(a, st);

@@ -286,10 +286,10 @@ int stoi_n_fr(int L);
 size_t stoi_ws_bytes(int n_clean, int n_pair, int L);
 cudaError_t launch_stoi(StoiArgs a, cudaStream_t st);
 
-// Hop blocks [j_begin, j_end) of the iSTFT of every signal (istft.cu).  Whole signals (carry == null): blocks
-// [0, T), the launcher drops those past L and splits the rest into chunks of fpc blocks, each of which recomputes
-// the frame before its first block.  A stream (disco_stream_istft): the blocks of frames t0 .. t0 + n_fr - 1, one
-// CTA per signal pair, the windowed half frame before them carried in `carry`.
+// Hop blocks [j_begin, j_end) of the iSTFT of every signal (istft.cu).  Whole signals (launch_istft, carry == null):
+// blocks [0, T), the launcher drops those past L and splits the rest into chunks of fpc blocks, each of which
+// recomputes the frame before its first block.  A stream (launch_stream_istft_slots, below): the blocks of frames
+// t0 .. t0 + n_fr - 1 of its record, one CTA per signal pair, the windowed half frame before them carried in `carry`.
 struct IstftArgs {
     const float2* Y;        // frame j of signal s at Y + (s * y_frames + j - y_t0) * F, frame-major complex64
     float* x;               // sample i of signal s at x[s * ld + i - x_first]
@@ -326,37 +326,43 @@ struct IstftLengthsKernel {
 };
 IstftLengthsKernel istft_lengths_kernel_for(int n_fft);
 
-// Streaming STFT (stream.cu): disco_stft on a signal that arrives chunk by chunk.
+// Streaming STFT (stream.cu): disco_stft on signals that arrive chunk by chunk, in n_slot independent streams (slots)
+// of n_sig signals each.  Slot s owns signals [s n_sig, (s + 1) n_sig) of every buffer and has the record below: from
+// the device array `slots` (a pool, disco_stream_stft_slots) or, with slots = null, `one` (n_slot = 1: a lockstep
+// stream, disco_stream_stft, whose record travels in the kernel parameters).
+struct StftSlot {
+    int length, n_new, t0, n_fr, blk_slot;
+    int final_call;         // 1: the stream ends at `length` (reflect padding at the end)
+    int hist_sel;           // the history buffer read (0 / 1)
+    int hist_write;         // 1: samples [length - N, length) are written to the other buffer
+};
+constexpr int kStftSlotFields = 8;   // ints per record of the C ABI
+static_assert(sizeof(StftSlot) == kStftSlotFields * sizeof(int), "StftSlot is the C ABI's record");
 struct StreamStftArgs {
-    const float* hist;      // [n_sig][N]: samples [L0 - N, L0) of every signal, L0 = length - n_new
-    const float* chunk;     // [n_sig][n_new]: samples [L0, length)
-    float* hist_out;        // [n_sig][N]: samples [length - N, length) written here (null: no update)
-    float2* Y;              // [n_sig][n_fr][F]: frames t0 .. t0 + n_fr - 1
-    float2* Y_blk;          // optional [n_sig][blk_frames][F]: the same frames at slots blk_slot ..
+    float* hist[2];         // two [n_slot][n_sig][N] buffers: samples [L0 - N, L0) in one, L0 = length - n_new
+    const float* chunk;     // [n_slot][n_sig][n_max]: samples [L0, length) at the start of each row
+    float2* Y;              // [n_slot][n_sig][f_max][F]: frames t0 .. t0 + n_fr - 1 at rows 0 .. n_fr - 1
+    float2* Y_blk;          // optional [n_slot][n_sig][blk_frames][F]: the same frames at rows blk_slot ..
     const float2* twiddle;  // [N/32][32]
     const float* window;    // [N]: 0.5 * periodic Hann
-    int n_sig, n_new, length, t0, n_fr, blk_frames, blk_slot;
-    int final_call;         // 1: the stream ends at `length` (reflect padding at the end)
+    const StftSlot* slots;  // [n_slot] device, or null: `one`
+    StftSlot one;
+    int n_slot, n_sig, n_max, f_max, blk_frames;
 };
-cudaError_t launch_stream_stft(const StreamStftArgs& a, int n_fft, cudaStream_t st);
-// A pool of independent streams (disco_stream_stft_slots): slot s owns signals [s n_sig, (s + 1) n_sig) and the record
-// slots[s][kStftSlotFields] = {length, n_new, t0, n_fr, blk_slot, final, hist_sel, hist_write}.  The slots kernel
-// takes this struct (stream_stft_kernel keeps StreamStftArgs and its parameter layout).  hist is [2][n_slot][n_sig][N]:
-// slot s reads buffer hist_sel and, with hist_write, writes its samples [length - N, length) to the other buffer;
-// chunk [n_slot][n_sig][n_max], Y [n_slot][n_sig][f_max][F], Y_blk [n_slot][n_sig][blk_frames][F].  The uniform
-// fields n_new, length, t0, n_fr, blk_slot, final_call and hist_out are not read.
-constexpr int kStftSlotFields = 8;
-struct StreamStftSlotsArgs : StreamStftArgs {
-    const int* slots;       // [n_slot][kStftSlotFields] device
-    int n_slot, n_max, f_max;
+// n_slot slots (a lockstep stream is one); no launch when nothing changes (a by-value record with no frames and no
+// history to write)
+cudaError_t launch_stream_stft_slots(const StreamStftArgs& a, int n_fft, cudaStream_t st);
+// The stream iSTFT (istft.cu): slot s runs istft_body on its signals [s n_sig, (s + 1) n_sig) with its record, from
+// `slots` (device, a pool) or, with slots = null, `one` (n_slot = 1, a lockstep stream).  a: Y [n_slot][n_sig]
+// [y_frames][F], carry [n_slot][n_sig][N/2], x [n_slot][n_sig][ld]; a.n_sig is the signals of one slot.  A slot with
+// n_fr = 0 that is not final is not run.
+struct IstftSlot {
+    int t0, n_fr, length, final_call, x_first;
 };
-cudaError_t launch_stream_stft_slots(const StreamStftSlotsArgs& a, int n_fft, cudaStream_t st);
-// The stream iSTFT of a pool (disco_stream_istft_slots, istft.cu): slot s runs istft_body on its signals [s n_sig,
-// (s + 1) n_sig) with the record slots[s][kIstftSlotFields] = {t0, n_fr, length, final, x_first}.  a: Y [n_slot]
-// [n_sig][y_frames][F], carry [n_slot][n_sig][N/2], x [n_slot][n_sig][ld]; a.n_sig is the signals of one slot.  A slot
-// with n_fr = 0 that is not final returns at once.
-constexpr int kIstftSlotFields = 5;
-cudaError_t launch_stream_istft_slots(const IstftArgs& a, const int* slots, int n_slot, int n_fft, cudaStream_t st);
+constexpr int kIstftSlotFields = 5;   // ints per record of the C ABI
+static_assert(sizeof(IstftSlot) == kIstftSlotFields * sizeof(int), "IstftSlot is the C ABI's record");
+cudaError_t launch_stream_istft_slots(const IstftArgs& a, const IstftSlot* slots, const IstftSlot& one, int n_slot,
+                                      int n_fft, cudaStream_t st);
 
 cudaError_t launch_tf_mask(const float2* S, const float2* Nn, float* M, size_t n, int kind, int power,
                            float thr_lin, cudaStream_t st);

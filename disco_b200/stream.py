@@ -13,7 +13,7 @@ Per push, for every run of newly completed frames (a run never crosses a block b
     mask_fn              the run's masks, kept in the open block's buffers
     scm_recursive        once a block's last masks are in: its statistics from the carried matrices,
     mwf_solve            and the block's filters W1_j, W2_j
-    stream_istft         the hop blocks of yf that became final (csrc/stream.cu)
+    stream_istft         the hop blocks of yf that became final (csrc/istft.cu)
 """
 import numpy as np
 import torch
@@ -43,6 +43,52 @@ def emission(length, n_fft=512, final=False):
     return T, (T - 1) * H
 
 
+
+def _check_params(n_fft, block, lambda_cor, lag):
+    """The checks OnlineTangoStream and OnlineTangoPool share, before their own channel limit."""
+    if n_fft not in N_FFTS:
+        raise ValueError("n_fft must be 256, 512 or 1024")
+    if not 1 <= int(block) <= 64:
+        raise ValueError("block must be 1..64 frames")
+    if not 0.0 <= float(lambda_cor) < 1.0:
+        raise ValueError("lambda_cor must be in [0, 1)")
+    if int(lag) == 0:
+        raise NotImplementedError("lag = 0 filters a frame with its own block's statistics, whose masks arrive "
+                                  "only after the block's later frames are out")
+    if int(lag) < 0:
+        raise ValueError("lag must be positive")
+
+
+def _check_ref_mic(ref_mic, C):
+    if not 0 <= int(ref_mic) < C:
+        raise ValueError("ref_mic must be in 0..C-1")
+
+
+def _cuda_device(device, what):
+    """torch.device of the CUDA device `device` (None or no index: the current one); `what` names the caller."""
+    device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+    if device.type != "cuda":
+        raise TypeError("the %s runs on a CUDA device, got %s" % (what, device))
+    if device.index is None:
+        device = torch.device("cuda", torch.cuda.current_device())
+    return device
+
+
+def _check_masks(masks, want, device):
+    """(mask_z, mask_w) of a mask_fn result: float32 tensors of shape `want` on `device` (mask_w = None: mask_z)."""
+    if not isinstance(masks, (tuple, list)) or len(masks) != 2:
+        raise ValueError("mask_fn must return the pair (mask_z, mask_w)")
+    mz, mw = masks
+    mw = mz if mw is None else mw
+    for m, name in ((mz, "mask_z"), (mw, "mask_w")):
+        if not isinstance(m, torch.Tensor):
+            raise ValueError("%s must be a tensor %s" % (name, want))
+        if tuple(m.shape) != want:
+            raise ValueError("%s shape %s, expected %s" % (name, tuple(m.shape), want))
+        if m.dtype != torch.float32 or m.device != device:
+            raise ValueError("%s must be float32 on %s" % (name, device))
+    return mz, mw
+
 class OnlineTangoStream:
     """B streams of K nodes x C microphones that start together and advance in lockstep; two-step recursive Tango
     (rank-`rank` GEVD filters), with the parameters of `online_tango`:
@@ -66,36 +112,19 @@ class OnlineTangoStream:
         B, K, C = int(B), int(K), int(C)
         if B < 1 or K < 1 or C < 1:
             raise ValueError("B, K and C must be positive")
-        if n_fft not in N_FFTS:
-            raise ValueError("n_fft must be 256, 512 or 1024")
-        if not 1 <= int(block) <= 64:
-            raise ValueError("block must be 1..64 frames")
-        if not 0.0 <= float(lambda_cor) < 1.0:
-            raise ValueError("lambda_cor must be in [0, 1)")
-        if int(lag) == 0:
-            raise NotImplementedError("lag = 0 filters a frame with its own block's statistics, whose masks arrive "
-                                      "only after the block's later frames are out")
-        if int(lag) < 0:
-            raise ValueError("lag must be positive")
+        _check_params(n_fft, block, lambda_cor, lag)
         D = C + K - 1
         if D > 8:
             raise NotImplementedError("the stream covers C + K - 1 <= 8 channels, got %d (the whole-signal "
                                       "online_tango goes to 16)" % D)
-        if not 0 <= int(ref_mic) < C:
-            raise ValueError("ref_mic must be in 0..C-1")
+        _check_ref_mic(ref_mic, C)
         if R0 is not None:
             if not isinstance(R0, (tuple, list)) or len(R0) != 2:
                 raise ValueError("R0 must be the pair (R_ss, R_nn)")
             for r in R0:
                 if not isinstance(r, torch.Tensor) or not r.is_cuda:
                     raise TypeError("R0 must hold CUDA tensors (disco_b200 has no CPU path)")
-        if device is None:
-            device = R0[0].device if R0 is not None else torch.device("cuda", torch.cuda.current_device())
-        device = torch.device(device)
-        if device.type != "cuda":
-            raise TypeError("the stream runs on a CUDA device, got %s" % device)
-        if device.index is None:
-            device = torch.device("cuda", torch.cuda.current_device())
+        device = _cuda_device(R0[0].device if device is None and R0 is not None else device, "stream")
         F, H, P = n_fft // 2 + 1, n_fft // 2, int(block)
         if R0 is not None:
             for r in R0:
@@ -196,21 +225,6 @@ class OnlineTangoStream:
         jw = j - self.lag
         return (stand_in, 1) if jw < 0 else (Ws[jw].unsqueeze(2), 0)
 
-    def _masks(self, masks, f):
-        if not isinstance(masks, (tuple, list)) or len(masks) != 2:
-            raise ValueError("mask_fn must return the pair (mask_z, mask_w)")
-        mz, mw = masks
-        mw = mz if mw is None else mw
-        want = (self.B, self.K, f, self.F)
-        for m, name in ((mz, "mask_z"), (mw, "mask_w")):
-            if not isinstance(m, torch.Tensor):
-                raise ValueError("%s must be a tensor %s" % (name, want))
-            if tuple(m.shape) != want:
-                raise ValueError("%s shape %s, expected %s" % (name, tuple(m.shape), want))
-            if m.dtype != torch.float32 or m.device != self.device:
-                raise ValueError("%s must be float32 on %s" % (name, self.device))
-        return mz, mw
-
     def _close_block(self, j, nb):
         """Statistics and filters of block j once the masks of its nb frames are in (nb < block: the final, partial
         block, whose recursion step is lambda^nb, as in the whole-signal scan)."""
@@ -249,7 +263,7 @@ class OnlineTangoStream:
             z, zn = ops.filter_sum_blocks(W, Y, None, P, lg, True, ref, n_fft)
             W, lg = self._in_force(self._W2s, self._pass2, j)
             yf, _ = ops.filter_sum_blocks(W, Y, z if K > 1 else None, P, lg, True, ref, n_fft)
-            mz, mw = self._masks(mask_fn(t, Y, z, zn), f)
+            mz, mw = _check_masks(mask_fn(t, Y, z, zn), (B, K, f, F), self.device)
             self._m1[:, :, slot:slot + f].copy_(mz)
             self._m2[:, :, slot:slot + f].copy_(mw)
             if K > 1:
@@ -317,29 +331,14 @@ class OnlineTangoPool:
         S, K, C = int(S), int(K), int(C)
         if S < 1 or K < 1 or C < 1:
             raise ValueError("S, K and C must be positive")
-        if n_fft not in N_FFTS:
-            raise ValueError("n_fft must be 256, 512 or 1024")
-        if not 1 <= int(block) <= 64:
-            raise ValueError("block must be 1..64 frames")
-        if not 0.0 <= float(lambda_cor) < 1.0:
-            raise ValueError("lambda_cor must be in [0, 1)")
-        if int(lag) == 0:
-            raise NotImplementedError("lag = 0 filters a frame with its own block's statistics, whose masks arrive "
-                                      "only after the block's later frames are out")
-        if int(lag) < 0:
-            raise ValueError("lag must be positive")
+        _check_params(n_fft, block, lambda_cor, lag)
         D = C + K - 1
         if D > 16:
             raise NotImplementedError("the pool covers C + K - 1 <= 16 channels, got %d" % D)
-        if not 0 <= int(ref_mic) < C:
-            raise ValueError("ref_mic must be in 0..C-1")
+        _check_ref_mic(ref_mic, C)
         if S > 65535:
             raise ValueError("at most 65535 slots")
-        device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
-        if device.type != "cuda":
-            raise TypeError("the pool runs on a CUDA device, got %s" % device)
-        if device.index is None:
-            device = torch.device("cuda", torch.cuda.current_device())
+        device = _cuda_device(device, "pool")
         self.S, self.K, self.C, self.D, self.F = S, K, C, D, n_fft // 2 + 1
         self.n_fft, self.block, self.lag = n_fft, int(block), int(lag)
         self.lambda_cor, self.mu, self.rank, self.ref_mic = float(lambda_cor), float(mu), rank, int(ref_mic)
@@ -508,21 +507,6 @@ class OnlineTangoPool:
             self._open[touched] = False
             raise
 
-    def _masks(self, masks, f):
-        if not isinstance(masks, (tuple, list)) or len(masks) != 2:
-            raise ValueError("mask_fn must return the pair (mask_z, mask_w)")
-        mz, mw = masks
-        mw = mz if mw is None else mw
-        want = (self.S, self.K, f, self.F)
-        for m, name in ((mz, "mask_z"), (mw, "mask_w")):
-            if not isinstance(m, torch.Tensor):
-                raise ValueError("%s must be a tensor %s" % (name, want))
-            if tuple(m.shape) != want:
-                raise ValueError("%s shape %s, expected %s" % (name, tuple(m.shape), want))
-            if m.dtype != torch.float32 or m.device != self.device:
-                raise ValueError("%s must be float32 on %s" % (name, self.device))
-        return mz, mw
-
     def _close_blocks(self, cl, nb, ci):
         """Statistics and filters of the open block of the slots `cl` (ci: the same indices on the device) once the
         masks of its nb[s] frames are in (nb < block: the final, partial block, whose recursion step is lambda^nb)."""
@@ -589,7 +573,7 @@ class OnlineTangoPool:
             else:
                 zf, znf, yff = (torch.zeros((S, K, f, F), **c64) for _ in range(3))
                 zf[ai], znf[ai], yff[ai] = z, zn, yf
-            mz, mw = self._masks(mask_fn(t0.copy(), nr.copy(), Y, zf, znf), f)
+            mz, mw = _check_masks(mask_fn(t0.copy(), nr.copy(), Y, zf, znf), (S, K, f, F), dev)
             self._m1[si, :, bi] = mz[si, :, ii]
             self._m2[si, :, bi] = mw[si, :, ii]
             if K > 1:

@@ -26,7 +26,8 @@ def sass(obj):
     for line in out.splitlines():
         m = re.match(r"\s+Function : (\S+)", line)
         if m:
-            cur = funcs.setdefault(m.group(1), [])
+            # a function in an anonymous namespace carries a hash of the source's path, which differs between the trees
+            cur = funcs.setdefault(re.sub(r"_GLOBAL__N__[0-9a-f]+_", "_GLOBAL__N__", m.group(1)), [])
             continue
         m = re.match(r"\s+/\*[0-9a-f]{4,}\*/\s+(.*?)\s*;", line)
         if cur is not None and m:
