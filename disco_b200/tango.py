@@ -139,6 +139,33 @@ def _step2_mask(vads, mods, mask_z, ch0_spectra, s0, n_fft, Y0=None, z=None, nod
     return _step1_mask(vads[1], None, ch0_spectra, s0, None, n_fft, lengths)
 
 
+def _check_sources(masks, s, n, vads, mask_for_z):
+    """The argument errors of an entry point that takes masks or the clean components s, n (tango_batched,
+    online.online_tango), raised before any device work."""
+    if mask_for_z is None:
+        raise TypeError("argument of type 'NoneType' is not iterable")   # reference tango.py:343
+    if masks is None and (s is None or n is None):
+        raise ValueError("either masks or the clean components (s, n) are required")
+    if (s is None or n is None) and mask_for_z in ("compressed", "use_oracle_refs", "use_oracle_zs"):
+        raise ValueError("mask_for_z=%r needs the clean components s and n" % mask_for_z)
+    if masks is None and "dnn" in [_mask_kind(v) for v in vads]:
+        raise ValueError("network masks ('crnn' / 'rnn') come in through masks=")
+    if mask_for_z == "use_oracle_sigs":
+        raise NotImplementedError(_ORACLE_SIGS)
+
+
+def _clean_masks(S, N, s, vads, ref_mic, n_fft, lengths=None):
+    """(mask_z, mask_w) [B, K, T, F] of the clean components: vads[0] of microphone ref_mic and vads[1] of microphone 0
+    (mask_z itself where they coincide) from their spectra S, N [B, K, C, T, F] or, for 'ivad', the signal s."""
+    spectra = lambda ch: (_ref_plane(S, ch), _ref_plane(N, ch))
+    mask_z = _step1_mask(vads[0], None, lambda: spectra(ref_mic), s[:, :, ref_mic], None, n_fft, lengths)
+    return mask_z, _step2_mask(vads, None, mask_z, lambda: spectra(0), s[:, :, 0], n_fft, ref_mic=ref_mic,
+                               lengths=lengths)
+
+
+_ORACLE_SIGS = "'use_oracle_sigs' is ill-formed in the reference (tango.py:423-427 indexes per-channel arrays by node)"
+
+
 def _z_for_stats(mask_for_z, vads, Z, mask_w, Zs, Zn, oracle_refs, clip=None):
     """What the other nodes contribute to the step-2 speech / noise statistics (tango.py:396-429): (z_rs, z_rn)
     [B, K, T, F] from the compressed signals Z, the step-2 masks mask_w, the filtered clean components Zs, Zn and
@@ -159,8 +186,7 @@ def _z_for_stats(mask_for_z, vads, Z, mask_w, Zs, Zn, oracle_refs, clip=None):
     if mask_for_z == "use_oracle_zs":
         return Zs, Zn
     if mask_for_z == "use_oracle_sigs":
-        raise NotImplementedError("'use_oracle_sigs' is ill-formed in the reference (tango.py:423-427 "
-                                  "indexes per-channel arrays by node)")
+        raise NotImplementedError(_ORACLE_SIGS)
     return Z, Z              # 'previous' and any other string: unmasked z in both statistics (tango.py:428-429)
 
 
@@ -256,30 +282,20 @@ def tango_batched(y, s=None, n=None, masks=None, vads=("irm1", "irm1"), mask_for
     T_b on.  Such a batch runs the routes that store the spectra (the fused STFT+SCM kernels assume one length);
     lengths=None or all lengths equal to L is the uniform batch, computed exactly as without the argument.
     """
-    if mask_for_z is None:
-        raise TypeError("argument of type 'NoneType' is not iterable")   # reference tango.py:343
+    _check_sources(masks, s, n, vads, mask_for_z)
     B, K, C, L = y.shape
     T, F = ops.n_frames(L, n_fft), n_fft // 2 + 1
     lens = _uneven_lengths(lengths, B, L, n_fft)
     stft = (lambda a: ops.stft(a, n_fft)) if lens is None else (lambda a: ops.stft_lengths(a, lens, n_fft))
     clip = None if lens is None else _frame_clip(lens, T, n_fft, y.device)
     oracle = masks is None
-    if oracle and (s is None or n is None):
-        raise ValueError("either masks or the clean components (s, n) are required")
     have_sn = s is not None and n is not None
-    if not have_sn and mask_for_z in ("compressed", "use_oracle_refs", "use_oracle_zs"):
-        raise ValueError("mask_for_z=%r needs the clean components s and n" % mask_for_z)
     S = N = None
     if have_sn and (oracle or diagnostics or "use_oracle_" in mask_for_z or mask_for_z == "compressed"):
         S, N = stft(s), stft(n)
     # ---- masks
     if oracle:
-        if "dnn" in [_mask_kind(v) for v in vads]:
-            raise ValueError("network masks ('crnn' / 'rnn') come in through masks=")
-        spectra = lambda ch: (_ref_plane(S, ch), _ref_plane(N, ch))
-        mask_z = _step1_mask(vads[0], None, lambda: spectra(ref_mic), s[:, :, ref_mic], None, n_fft, lens)
-        mask_w = _step2_mask(vads, None, mask_z, lambda: spectra(0), s[:, :, 0], n_fft, ref_mic=ref_mic,
-                             lengths=lens)
+        mask_z, mask_w = _clean_masks(S, N, s, vads, ref_mic, n_fft, lens)
     else:
         mask_z, mask_w = masks
         if mask_w is None:
