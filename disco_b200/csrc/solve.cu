@@ -145,12 +145,24 @@ DISCO_DEV void g_jacobi(cd* A, cd* V, Rot* rot, int l, unsigned gm) {
     }
     const double tot = gsum<G>(mine, gm);
     __syncwarp(gm);
+    // Converged when the off-diagonal energy is below 1e-26 of the total AND every pair is small next to its own
+    // diagonal: |a_pq|^2 <= 1e-26 |a_pp a_qq| + 1e-32 ||A||_F^2.  The first rule alone leaves entries of 1e-13 ||A||,
+    // an absolute error of every eigenpair; where an ill-conditioned Rnn puts ||A|| near 1e9, the small eigenpairs that
+    // 'full' and rank > 1 sum were off by 1e-4.  The pair rule gives them relative accuracy; its 1e-32 floor (1e-16
+    // ||A||, the float64 rounding of A) ends the sweeps on the rounding noise of a singular A.  Entries below 1e-300,
+    // which no rotation touches, never hold the sweeps.  tot = inf (Rnn == 0 puts A near 1e300 Rss, so norm2
+    // overflows) stops before the first sweep, as it always did: both rules hold with inf on the right.
     for (int sweep = 0; sweep < 40; ++sweep) {
         double offm = 0.0;
+        bool loose = false;
         if (act)
-            for (int j = l + 1; j < D; ++j) offm += norm2(A[l * P + j]);
+            for (int j = l + 1; j < D; ++j) {
+                const double n2 = norm2(A[l * P + j]);
+                offm += n2;
+                loose |= n2 >= 1e-300 && n2 > 1e-26 * fabs(A[l * P + l].x) * fabs(A[j * P + j].x) + 1e-32 * tot;
+            }
         const double off = gsum<G>(offm, gm);
-        if (off <= 1e-26 * tot) break;          // group-uniform
+        if (off <= 1e-26 * tot && !__any_sync(gm, loose)) break;   // group-uniform
         for (int r = 0; r < N - 1; ++r) {
             if (l < NP) {                        // lane l owns pair l of this round (circle method)
                 int a0, b0;
@@ -170,7 +182,7 @@ DISCO_DEV void g_jacobi(cd* A, cd* V, Rot* rot, int l, unsigned gm) {
                 if (q < D) {                     // q >= D: the dummy player of an odd D
                     const cd b = A[p * P + q];
                     const double n2 = norm2(b);
-                    if (n2 >= 1e-300) {
+                    if (n2 >= 1e-300 && n2 <= 1.7976931348623157e308) {   // inf: ab = n2 rsqrt(n2) is inf * 0
                         const double inv_ab = rsqrt(n2), ab = n2 * inv_ab;
                         const cd ph = inv_ab * b;
                         const double d = 0.5 * (A[q * P + q].x - A[p * P + p].x);

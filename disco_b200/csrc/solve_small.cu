@@ -71,7 +71,7 @@ template <int D>
 DISCO_DEV void jacobi_rotate(cd (&A)[D][Ld<D>::v], cd (&V)[D][Ld<D>::v], int p, int q) {
     const cd b = A[p][q];
     const double n2 = norm2(b);
-    if (n2 < 1e-300) return;
+    if (n2 < 1e-300 || n2 > 1.7976931348623157e308) return;   // inf: ab = n2 rsqrt(n2) is inf * 0
     const double inv_ab = rsqrt(n2), ab = n2 * inv_ab;
     const cd ph = inv_ab * b;
     const double d = 0.5 * (A[q][q].x - A[p][p].x);
@@ -104,7 +104,9 @@ DISCO_DEV void jacobi_rotate(cd (&A)[D][Ld<D>::v], cd (&V)[D][Ld<D>::v], int p, 
 
 // Cyclic Jacobi for a Hermitian matrix A (destroyed); V receives the eigenvectors (columns),
 // lam the eigenvalues (unsorted).  Converged when the off-diagonal energy is below 1e-26 of the
-// total (the inputs carry float32 rounding, ~1e-14 relative energy).  For D <= 4 the (p, q) loops are
+// total (the inputs carry float32 rounding, ~1e-14 relative energy) and every pair is small next to its own diagonal,
+// |a_pq|^2 <= 1e-26 |a_pp a_qq| + 1e-32 ||A||_F^2, which gives the small eigenpairs relative accuracy (solve.cu
+// g_jacobi).  For D <= 4 the (p, q) loops are
 // fully unrolled so that A and V live in registers; larger matrices index local memory.
 template <int D>
 DISCO_DEV void jacobi(cd (&A)[D][Ld<D>::v], cd (&V)[D][Ld<D>::v], double (&lam)[D]) {
@@ -120,11 +122,16 @@ DISCO_DEV void jacobi(cd (&A)[D][Ld<D>::v], cd (&V)[D][Ld<D>::v], double (&lam)[
 #pragma unroll 1
     for (int sweep = 0; sweep < 30; ++sweep) {
         double off = 0.0;
+        bool loose = false;
 #pragma unroll
         for (int p = 0; p < D; ++p)
 #pragma unroll
-            for (int q = p + 1; q < D; ++q) off += norm2(A[p][q]);
-        if (off <= 1e-26 * tot) break;
+            for (int q = p + 1; q < D; ++q) {
+                const double n2 = norm2(A[p][q]);
+                off += n2;
+                loose |= n2 >= 1e-300 && n2 > 1e-26 * fabs(A[p][p].x) * fabs(A[q][q].x) + 1e-32 * tot;
+            }
+        if (off <= 1e-26 * tot && !loose) break;
         if constexpr (D <= 4) {
 #pragma unroll
             for (int p = 0; p < D - 1; ++p)

@@ -11,10 +11,11 @@ import torch
 
 from conftest import rel_l2
 from oracle import solve_f64
+from test_gpu_solver_instances import ALL_D, mpb
 
 pytestmark = pytest.mark.gpu
 
-DS = [1, 2, 3, 4, 5, 7, 8, 9, 12, 16]
+DS = list(ALL_D)        # every instantiation of both engines (tests/test_gpu_solver_instances.py INSTANCES)
 EPS64 = np.finfo(np.float64).eps
 FILTERS = [("gevd", 1, 1.0), ("gevd", 2, 2.5), ("gevd", "full", 1.0), ("r1-mwf", 1, 2.5), ("mwf", 1, 1.0)]
 
@@ -78,14 +79,23 @@ def _err_bound(cond, gap, D):
     return 2e-6 + 10 * D * cond * EPS64 / gap + cond * 1e-13
 
 
+def _cond_draws(seeds):
+    """(generator, cond) for cond = 1 ... 1e10 under each seed, one generator per seed drawn in that order."""
+    for seed in seeds:
+        rng = np.random.default_rng(seed)
+        for cond in (1e0, 1e2, 1e4, 1e6, 1e8, 1e10):
+            yield rng, cond
+
+
 @pytest.mark.parametrize("D", DS)
 def test_conditioning(dev, D):
     """cond(Rnn) = 1 ... 1e10 as constructed.  Rounding to complex64 perturbs Rnn by ~6e-8 of its norm, so from
     cond ~1e7 on the matrix the solver sees has its own (larger, or no) condition number: the forward check takes
     only the bins whose complex64 Rnn keeps lambda_min >= 1e-10 tr (far above the 1e-13 pivot floor), with
-    kappa of those matrices in the bound, and requires every other bin to be finite."""
-    rng = np.random.default_rng(100 + D)
-    for cond in (1e0, 1e2, 1e4, 1e6, 1e8, 1e10):
+    kappa of those matrices in the bound, and requires every other bin to be finite.  Two draws per D: 'full' also
+    sums the small eigenpairs of the whitened matrix, whose norm reaches 1e9 here, so it checks that the Jacobi sweeps
+    resolve them relative to their own size (at D = 11 and 15 they did not before the per-pair stopping rule)."""
+    for rng, cond in _cond_draws((100 + D, 1700 + D)):
         Rss, Rnn = _cond_family(rng, 48, D, cond)
         Rss, Rnn = _c64h(Rss), _c64h(Rnn)
         ev = np.linalg.eigvalsh(Rnn.astype(complex))
@@ -110,7 +120,7 @@ def test_conditioning(dev, D):
                 assert rel_l2(T1[ok], t1) <= tol, (cond, typ, rank, rel_l2(T1[ok], t1), tol)
 
 
-@pytest.mark.parametrize("D", [1, 2, 3, 4, 5, 7, 8])
+@pytest.mark.parametrize("D", DS)
 def test_small_pivot_is_used_as_is(dev, D):
     """A Cholesky pivot of 1.2e-10 tr(Rnn), a thousand times above the 1e-13 tr / D floor, is used as it is:
     Rnn = diag(1, ..., 1, p) with p exact in complex64, generic Rss.  'full' is left out: its Jacobi sweeps stop
@@ -426,27 +436,23 @@ def test_non_hermitian_input_is_symmetrised(dev, D):
         assert np.array_equal(Wh, Wr) and np.array_equal(Th, Tr), (typ, rank)
 
 
-def _mpb(D):
-    return 64 if D <= 4 else (16 if D <= 8 else 4)
-
-
 @pytest.mark.parametrize("D", DS)
 def test_batch_tails(dev, D):
     """disco_mwf_solve with W / T1 longer than n_mat * D and filled with a sentinel: the tail stays untouched,
     n_mat = 0 is a no-op, and the solved part equals the solve of exactly those matrices."""
     from disco_b200 import _lib, ops
     lib = _lib.load()
-    mpb = _mpb(D)
+    mpb_ = mpb(D)
     rng = np.random.default_rng(900 + D)
-    many = 3 * mpb + 5
+    many = 3 * mpb_ + 5
     Rss, Rnn = _cond_family(rng, many, D, 1e2)
     Rs, Rn = torch.from_numpy(_c64(Rss)).to(dev), torch.from_numpy(_c64(Rnn)).to(dev)
     ref_W, ref_T = ops.mwf_solve(Rs, Rn, 1.0, "gevd", 1)
     sentinel = torch.view_as_complex(torch.full((many * D + 3 * D, 2), float.fromhex("0x1.5p-7"), device=dev))
     ptr = lambda t: ctypes.c_void_p(t.data_ptr())
     stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-    for n_mat in sorted({0, 1, mpb - 1, mpb, mpb + 1, many}):
-        if n_mat == 0 and mpb == 1:
+    for n_mat in sorted({0, 1, mpb_ - 1, mpb_, mpb_ + 1, many}):
+        if n_mat == 0 and mpb_ == 1:
             continue
         W, T = sentinel.clone(), sentinel.clone()
         assert lib.disco_mwf_solve(ptr(Rs), ptr(Rn), ptr(W), ptr(T), n_mat, D, 0, 1, ctypes.c_double(1.0), stream) == 0
