@@ -5,6 +5,7 @@ arithmetic happens in the hand-written kernels.
 Layouts: spectra are frame-major ``[..., T, F]`` complex64; ``layout='FT'`` arguments select the
 reference's NumPy layout ``[..., F, T]`` for masks / final outputs (SURVEY.md §8b op table).
 """
+import collections
 import ctypes
 import math
 
@@ -72,6 +73,35 @@ def _need(t, dtype, name):
     return t
 
 
+def _bins(F, n_fft, name):
+    """Spectra handed to a kernel hold n_fft / 2 + 1 bins: the library derives F from n_fft alone."""
+    if F != n_fft // 2 + 1:
+        raise ValueError("%s has %d bins, n_fft=%d needs %d" % (name, F, n_fft, n_fft // 2 + 1))
+
+
+# What a workspace of stft_scm(keep_partials=True) / stft_scm2 was written with: its consumers read the per-segment
+# partial sums with the launch plan of these sizes AND of the reserved-SM setting current when they run.
+WorkspacePlan = collections.namedtuple("WorkspacePlan", "G C L n_fft n_set reserved_sms")
+_reserved_sms = 0     # the value last given to set_reserved_sms (the library's setting is process-wide)
+
+
+def _workspace(ws, G, C, L, n_fft, n_set):
+    """Check that `ws` is a workspace written for (G, C, L, n_fft, n_set) under the current reserved-SM setting and
+    holds the bytes its consumers read."""
+    _need(ws, torch.float32, "ws")
+    plan = getattr(ws, "disco_plan", None)
+    if not isinstance(plan, WorkspacePlan):
+        raise ValueError("ws is not a workspace returned by stft_scm(keep_partials=True) or stft_scm2")
+    want = WorkspacePlan(int(G), int(C), int(L), int(n_fft), int(n_set), _reserved_sms)
+    if plan != want:
+        raise ValueError("workspace written for %s, read as %s" % (tuple(plan), tuple(want)))
+    lib = _lib.load()
+    size = lib.disco_stft_scm_workspace if n_set == 1 else lib.disco_stft_scm2_workspace
+    need = size(int(G), int(C), int(L), int(n_fft))
+    if ws.numel() * ws.element_size() < need:
+        raise ValueError("workspace holds %d bytes, %d needed" % (ws.numel() * ws.element_size(), need))
+
+
 def n_frames(length, n_fft=512):
     """1 + L // hop (reference tango.py:287)."""
     return 1 + length // (n_fft // 2)
@@ -86,6 +116,8 @@ def init(n_fft=512):
 def stft(x, n_fft=512):
     """x [..., L] float32 -> Y [..., T, F] complex64 (librosa center/reflect/periodic-Hann semantics)."""
     _need(x, torch.float32, "x")
+    if x.dim() < 1:
+        raise ValueError("x must be [..., samples]")
     L = x.shape[-1]
     n_sig = x.numel() // L
     T, F = n_frames(L, n_fft), n_fft // 2 + 1
@@ -119,6 +151,7 @@ def stft_scm(x, mask, n_fft=512, mask_layout="TF", keep_partials=False):
     if keep_partials:
         _lib.check(lib.disco_stft_scm(_ptr(x), _ptr(mask), lay, _ptr(Y), None, None, G, C, L, n_fft,
                                       _ptr(ws), ws_bytes, _stream()))
+        ws.disco_plan = WorkspacePlan(G, C, L, int(n_fft), 1, _reserved_sms)
         return Y, ws
     Rss = torch.empty((G, F, C, C), dtype=torch.complex64, device=x.device)
     Rnn = torch.empty_like(Rss)
@@ -132,6 +165,7 @@ def mwf_solve_workspace(ws, G, C, L, n_fft=512, mu=1.0, type="gevd", rank=1, wan
     """mwf_solve on the SCMs a preceding stft_scm(..., keep_partials=True) left in `ws`.
     Returns W, t1 [G, F, C] (and Rss, Rnn [G, F, C, C] when want_scm)."""
     ftype, r = _filter_args(type, rank)
+    _workspace(ws, G, C, L, n_fft, 1)
     F = n_fft // 2 + 1
     W = torch.empty((G, F, C), dtype=torch.complex64, device=ws.device)
     T1 = torch.empty_like(W)
@@ -145,8 +179,13 @@ def mwf_solve_workspace(ws, G, C, L, n_fft=512, mu=1.0, type="gevd", rank=1, wan
 
 
 def set_reserved_sms(n):
-    """Leave n SMs free of the persistent fused STFT+SCM kernel (room for a concurrent NCCL collective)."""
+    """Leave n SMs free of the persistent fused STFT+SCM kernel (room for a concurrent NCCL collective).  A workspace
+    is consumed under the setting it was written with (the consumers refuse it otherwise).  The setting is tracked
+    here: a direct call of the library's disco_set_reserved_sms bypasses it, and a workspace written and consumed
+    after such a call is then only checked for its sizes and byte count."""
+    global _reserved_sms
     _lib.check(_lib.load().disco_set_reserved_sms(int(n)))
+    _reserved_sms = int(n)
 
 
 def stft_scm_supported(n_fft, C, n_mask=1):
@@ -180,12 +219,14 @@ def stft_scm2(x, mask_a, mask_b, n_fft=512, mask_layout="TF", want_Y=True):
     ws = torch.empty(max(ws_bytes, 16) // 4, dtype=torch.float32, device=x.device)
     _lib.check(lib.disco_stft_scm2(_ptr(x), _ptr(mask_a), _ptr(mask_b), lay, _ptr(Y), G, C, L, n_fft, _ptr(ws),
                                    ws_bytes, _stream()))
+    ws.disco_plan = WorkspacePlan(G, C, L, int(n_fft), 2, _reserved_sms)
     return Y, ws
 
 
 @_on_device
 def scm_from_workspace(ws, G, C, L, n_fft=512, n_set=1, set=0):
     """Rss, Rnn [G, F, C, C] of mask set `set` from the partial sums a fused STFT+SCM call left in `ws`."""
+    _workspace(ws, G, C, L, n_fft, n_set)
     F = n_fft // 2 + 1
     Rss = torch.empty((G, F, C, C), dtype=torch.complex64, device=ws.device)
     Rnn = torch.empty_like(Rss)
@@ -198,6 +239,7 @@ def scm_from_workspace(ws, G, C, L, n_fft=512, n_set=1, set=0):
 def mwf_solve_workspace2(ws, G, C, L, n_fft=512, mu=1.0, type="gevd", rank=1):
     """Both filter sets of a stft_scm2 workspace in one launch: W, t1 [2, G, F, C] (0: mask_a, 1: mask_b)."""
     ftype, r = _filter_args(type, rank)
+    _workspace(ws, G, C, L, n_fft, 2)
     F = n_fft // 2 + 1
     W = torch.empty((2, G, F, C), dtype=torch.complex64, device=ws.device)
     T1 = torch.empty_like(W)
@@ -214,7 +256,10 @@ def filter_dual(W1, W2, Y, ref=0, n_fft=512, out_layout="TF", want_zn=True):
     _need(W1, torch.complex64, "W1")
     _need(W2, torch.complex64, "W2")
     _need(Y, torch.complex64, "Y")
+    if Y.dim() < 3:
+        raise ValueError("Y must be [..., C, T, F]")
     C, T, F = Y.shape[-3:]
+    _bins(F, n_fft, "Y")
     lead = tuple(Y.shape[:-3])
     G = Y.numel() // (C * T * F)
     if tuple(W1.shape) != lead + (F, C) or tuple(W2.shape) != lead + (F, C):
@@ -277,6 +322,8 @@ def _cat_geometry(y_shape, z_shape=None, node_sel=None, z_layout="BK"):
     z_layout 'BK', node-major (K, B, T, F) with 'KB' (what an all-gather over node-owning ranks delivers,
     disco_b200/dist.py), or None: no exchange, every (b, k) is an independent single-node problem.  node_sel: the
     nodes Y holds (None = all K).  Returns n_utt, K, sel (ctypes int array or None), n_sel, z_layout flag."""
+    if len(y_shape) != 5:
+        raise ValueError("Y shape %s, expected [B, Ksel, C, T, F]" % (tuple(y_shape),))
     B, Ks, C, T, F = y_shape
     if z_shape is None:
         return B * Ks, 1, None, 1, 0
@@ -294,11 +341,13 @@ def _cat_geometry(y_shape, z_shape=None, node_sel=None, z_layout="BK"):
     return B, K, sel, n_sel, (0 if z_layout == "BK" else 1)
 
 
-def _cat_args(Y, Z, node_sel, z_layout="BK"):
-    """_cat_geometry of the tensors Y (complex64, [B, Ksel, C, T, F]) and Z (complex64 or None)."""
+def _cat_args(Y, Z, node_sel, n_fft, z_layout="BK"):
+    """_cat_geometry of the tensors Y (complex64, [B, Ksel, C, T, F], F = n_fft / 2 + 1) and Z (complex64 or None)."""
     _need(Y, torch.complex64, "Y")
     if Z is not None:
         _need(Z, torch.complex64, "Z")
+    if Y.dim() == 5:
+        _bins(Y.shape[-1], n_fft, "Y")
     return _cat_geometry(tuple(Y.shape), None if Z is None else tuple(Z.shape), node_sel, z_layout)
 
 
@@ -314,7 +363,7 @@ def masked_scm(Y, mask, Z=None, n_fft=512, mask_layout="TF", node_sel=None, z_la
     """Y [B, Ksel, C, T, F], Z [B, K, T, F] (or [K, B, T, F] with z_layout='KB') or None (K = 1),
     mask [B, Ksel, T, F] / [B, Ksel, F, T] or None
     -> Rss, Rnn [B, Ksel, F, D, D], D = C + K - 1 (own mics, then z of the other nodes)."""
-    n_utt, K, sel, n_sel, zl = _cat_args(Y, Z, node_sel, z_layout)
+    n_utt, K, sel, n_sel, zl = _cat_args(Y, Z, node_sel, n_fft, z_layout)
     B, Ks, C, T, F = Y.shape
     lay = _layout(mask_layout)
     if mask is not None:
@@ -338,7 +387,10 @@ def filter_sum_scm(W1, Y, mask, ref=0, n_fft=512, mask_layout="TF"):
     _need(W1, torch.complex64, "W1")
     _need(Y, torch.complex64, "Y")
     _need(mask, torch.float32, "mask")
+    if Y.dim() < 3:
+        raise ValueError("Y must be [..., C, T, F]")
     C, T, F = Y.shape[-3:]
+    _bins(F, n_fft, "Y")
     lead = Y.shape[:-3]
     G = Y.numel() // (C * T * F)
     lay = _layout(mask_layout)
@@ -367,10 +419,14 @@ def tango_mid(W1, Y, mask_w, ref=0, n_fft=512):
     _need(W1, torch.complex64, "W1")
     _need(Y, torch.complex64, "Y")
     _need(mask_w, torch.float32, "mask_w")
+    if Y.dim() != 5:
+        raise ValueError("Y must be [B, K, C, T, F]")
     B, K, C, T, F = Y.shape
+    _bins(F, n_fft, "Y")
     D = C + K - 1
     if tuple(W1.shape) != (B, K, F, C) or tuple(mask_w.shape) != (B, K, T, F):
-        raise ValueError("shape mismatch")
+        raise ValueError("W1 %s / mask_w %s, expected %s / %s" % (tuple(W1.shape), tuple(mask_w.shape), (B, K, F, C),
+                                                                  (B, K, T, F)))
     z = torch.empty((B, K, T, F), dtype=torch.complex64, device=Y.device)
     zn = torch.empty_like(z)
     Rss = torch.empty((B, K, F, D, D), dtype=torch.complex64, device=Y.device)
@@ -387,6 +443,8 @@ def mwf_solve(Rss, Rnn, mu=1.0, type="gevd", rank=1):
     _need(Rss, torch.complex64, "Rss")
     _need(Rnn, torch.complex64, "Rnn")
     ftype, r = _filter_args(type, rank)
+    if Rss.dim() < 2 or Rss.shape[-1] != Rss.shape[-2] or Rnn.shape != Rss.shape:
+        raise ValueError("Rss %s / Rnn %s, expected two [..., D, D]" % (tuple(Rss.shape), tuple(Rnn.shape)))
     D = Rss.shape[-1]
     n_mat = Rss.numel() // (D * D)
     W = torch.empty(Rss.shape[:-1], dtype=torch.complex64, device=Rss.device)
@@ -402,7 +460,7 @@ def filter_sum(W, Y, Z=None, conj=True, ref=None, n_fft=512, out_layout="TF", no
     W [B, Ksel, F, D]; Z [B, K, T, F] (or [K, B, T, F] with z_layout='KB');
     returns out (and resid = x[ref] - out when ref is given), [B, Ksel, T, F] or [.., F, T]."""
     _need(W, torch.complex64, "W")
-    n_utt, K, sel, n_sel, zl = _cat_args(Y, Z, node_sel, z_layout)
+    n_utt, K, sel, n_sel, zl = _cat_args(Y, Z, node_sel, n_fft, z_layout)
     B, Ks, C, T, F = Y.shape
     D = C + K - 1
     if tuple(W.shape) != (B, Ks, F, D):
@@ -502,7 +560,7 @@ def scm_recursive(Y, mask, Z=None, lambda_cor=0.95, block=8, power=2, R0=None, n
     frames: None, or host integers, one per utterance in [1, T]: utterance b then has frames[b] frames, its blocks
     j < ceil(frames[b] / block) equal the call on Y[b, ..., :frames[b], :] alone bit for bit, its later blocks are 0,
     and no frame from frames[b] on is read."""
-    n_utt, K, sel, n_sel, _ = _cat_args(Y, Z, node_sel)
+    n_utt, K, sel, n_sel, _ = _cat_args(Y, Z, node_sel, n_fft)
     if mask is not None:
         _need(mask, torch.float32, "mask")
     B, Ks, C, T, F = Y.shape
@@ -539,7 +597,7 @@ def filter_sum_blocks(W, Y, Z=None, block=8, lag=1, conj=True, ref=0, n_fft=512,
     frames: None, or host integers, one per utterance in [1, T]: frames t < frames[b] of utterance b are the call on
     its first frames[b] frames alone (reading only W[b, :, :ceil(frames[b] / block)]); later frames are 0."""
     _need(W, torch.complex64, "W")
-    n_utt, K, sel, n_sel, _ = _cat_args(Y, Z, node_sel)
+    n_utt, K, sel, n_sel, _ = _cat_args(Y, Z, node_sel, n_fft)
     B, Ks, C, T, F = Y.shape
     D, J = C + K - 1, (T + block - 1) // block
     if tuple(W.shape) != (B, Ks, J, F, D):
@@ -716,6 +774,8 @@ def band_stats(x, ba, sel=None):
             raise ValueError("sel must have the shape of x")
         sv = torch.empty_strided(xv.shape, (ld, 1), dtype=torch.float32, device=x.device)
         sv.copy_(sel.reshape(-1, L))
+    if not isinstance(ba, torch.Tensor) or ba.is_complex():
+        raise TypeError("ba must be a real tensor [n_band, 2, order + 1]")
     ba = ba.to(device=x.device, dtype=torch.float64).contiguous()
     if ba.dim() != 3 or ba.shape[1] != 2:
         raise ValueError("ba must be [n_band, 2, order + 1]")

@@ -132,6 +132,10 @@ DISCO_API int disco_stft_scm2(const float* x, const float* mask_a, const float* 
  * C <= 4, n_fft in {256, 512} (disco_stft_scm_supported(n_fft, C, 2)). */
 DISCO_API int disco_stft_filter_dual(const float* x, const void* W1, const void* W2, void* z, void* zn, void* yf,
                                      int ref, int out_layout, int n_grp, int C, int length, int n_fft, void* stream);
+/* disco_scm_from_workspace: Rss, Rnn [n_grp][F][C][C] complex64 out.  It reads disco_stft_scm_workspace() (n_set = 1)
+ * or disco_stft_scm2_workspace() (n_set = 2) bytes of `workspace` for (n_grp, C, length, n_fft), laid out by the launch
+ * plan of the reserved-SM setting current at the call: the workspace must have been written with the same arguments
+ * under the same setting (the library receives no byte count to check). */
 DISCO_API int disco_scm_from_workspace(const void* workspace, int n_set, int set, void* Rss, void* Rnn, int n_grp,
                              int C, int length, int n_fft, void* stream);
 
@@ -151,6 +155,8 @@ DISCO_API int disco_tf_mask(const void* S, const void* N, float* M, size_t n_ele
  * indices that have C microphones (Y, mask, outputs then hold n_utt * n_sel groups);
  * node_sel == NULL means all K nodes.
  *   Y [n_utt*K][C][T][F], Z [n_utt][K][T][F] complex64; mask [n_utt*K] planes; Rss/Rnn [n_utt*K][F][D][D]
+ *   (with node_sel: n_utt*n_sel groups in Y, mask and the outputs; Z keeps all K nodes).  F = n_fft/2 + 1 always:
+ *   spectra of another bin count are read past their end.
  * z_layout = DISCO_Z_NODE_MAJOR reads Z as [K][n_utt][T][F] -- the buffer an NCCL all-gather over node-owning
  * ranks fills (the reference's exchange, tango.py:379-386) -- so the gathered signals are never transposed. */
 DISCO_API int disco_masked_scm(const void* Y, const void* Z, const float* mask, int mask_layout, void* Rss, void* Rnn,
@@ -187,7 +193,9 @@ DISCO_API int disco_mwf_solve(const void* Rss, const void* Rnn, void* W, void* T
 
 /* Same solve, reading the SCMs from the workspace a preceding disco_stft_scm(n_grp, C, length, n_fft) call
  * left behind (matrix index = group * F + bin; W, T1 [n_grp][F][C]).  Rss / Rnn non-NULL: also write the
- * matrices ([n_grp][F][C][C]). */
+ * matrices ([n_grp][F][C][C]).  It reads disco_stft_scm_workspace(n_grp, C, length, n_fft) bytes of `workspace` (two
+ * sets: disco_stft_scm2_workspace()) as laid out under the current disco_set_reserved_sms value, which must be the one
+ * the workspace was written under. */
 DISCO_API int disco_mwf_solve_workspace(const void* workspace, void* W, void* T1, void* Rss, void* Rnn, int n_grp,
                                         int C, int length, int n_fft, int filter_type, int rank, double mu,
                                         void* stream);
@@ -201,7 +209,8 @@ DISCO_API int disco_mwf_solve_workspace2(const void* workspace, void* W, void* T
  * Replaces np.inner(conj(w), x[:, f, t]) (conj_w = 1) / np.inner(t1, x[:, f, t]) (conj_w = 0) over
  * all (f, t) (reference tango.py:369-374, 445-450) on the same concatenated channel view as
  * disco_masked_scm, and optionally resid = x[ref] - out (zn, tango.py:376).
- *   W [n_utt*K][F][D]; out, resid [n_utt*K] planes in `out_layout` (resid may be NULL) */
+ *   W [n_utt*K][F][D]; Y, Z as disco_masked_scm; out, resid [n_utt*K] planes in `out_layout` (resid may be NULL);
+ *   n_utt*n_sel groups with node_sel */
 DISCO_API int disco_filter_sum(const void* W, int conj_w, const void* Y, const void* Z, void* out, void* resid, int ref,
                      int out_layout, int n_utt, int K, int C, int T, int n_fft, const int* node_sel, int n_sel,
                      int z_layout, void* stream);
@@ -252,7 +261,8 @@ DISCO_API int disco_istft_lengths(const void* Y, const int* lengths, const int* 
  *   R0ss, R0nn: optional initial matrices [n_utt*n_sel][F][D][D] (NULL = zeros), Hermitian.  At D <= 8 every entry
  *   is read; at D >= 9 only the upper triangle (r <= c) and of the diagonal only the real part, the rest is taken
  *   as the conjugate mirror and 0.  (Both agree on an exactly Hermitian R0 with a real diagonal.)
- * disco_filter_sum_blocks applies one filter per block: frame t gets W[.., t / block - lag, ..]
+ * disco_filter_sum_blocks applies one filter per block, W [n_utt*n_sel][J][F][D]; out, resid [n_utt*n_sel][T][F]
+ * (Y, Z as disco_masked_scm): frame t gets W[.., t / block - lag, ..]
  * (lag = 1: the filter of the last completed block, strictly causal; while that index is negative the
  * reference channel passes through), out = w^H x (conj_w = 1), resid = x[ref] - out (optional). */
 DISCO_API int disco_scm_recursive(const void* Y, const void* Z, const float* mask, const void* R0ss, const void* R0nn,
