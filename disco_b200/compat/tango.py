@@ -1,6 +1,7 @@
-"""Names of disco_theque/speech_enhancement/tango.py (:28-36, :142-240, :252-457)."""
+"""Names of disco_theque/speech_enhancement/tango.py (:28-36, :41-139, :142-240, :252-457, :460-641)."""
 import numpy as np
 
+from ..evaluate import get_dset, get_directory_name, get_input_signals, load_models, main  # noqa: F401  (tango.py:41-139, 460)
 from ..tango import offline_tango  # noqa: F401  (reference signature, tango.py:252)
 from ._util import DEVICE
 from .sigproc_utils import tf_mask, vad_oracle_batch
