@@ -1,8 +1,10 @@
 """Step-1-only variant of Tango (disco_theque/speech_enhancement/get_z_signals.py:213-317): produces the
-compressed signals that are saved as DNN training inputs (get_z_signals.py:350-359)."""
+compressed signals that are saved as DNN training inputs (get_z_signals.py:350-359).  main and its helpers
+(get_z_signals.py:30-120, 320-360) are those of the batched driver, disco_b200.get_z."""
 import torch
 
 from .. import ops
+from ..get_z import get_dset, get_directory_name, get_input_signals, load_models, main  # noqa: F401  (:30-120, 320)
 from ..tango import _ref_plane, _reference_lists, _step1_mask, _to_dev, tango_step1
 
 

@@ -63,20 +63,11 @@ def _read(path):
     return wav_io.read(path, dtype="float32")
 
 
-def get_input_signals(i_rir, scenario="living", noise="ssn", snr_range=None, *, path_to_dataset=PATH_TO_DATASET,
-                      nb_ch=(4, 4, 4, 4)):
-    """tango.py:55-111: the convolved target, noise and mixture of every microphone of RIR i_rir (lists [node][ch]
-    of float32 arrays), the dry target and noise, the sampling rate and the mixing SNR stored with the data set.
-    n_dry is scaled by that SNR in float32, as the reference's in-place `*=` on its float32 array does.
-    Every convolved file must have the length and rate of the first and the dry files its rate: ValueError naming
-    the file otherwise; a missing file raises FileNotFoundError with its path."""
-    path_to_set = os.path.join(path_to_dataset, "disco", scenario, get_dset(i_rir))
-    dirry = get_directory_name([[0, 6]] if snr_range is None else snr_range)
-    snr_file = os.path.join(path_to_set, "log", "snrs", "dry", dirry, "") + "{}_{}.npy".format(str(i_rir), noise)
-    if not os.path.isfile(snr_file):
-        raise FileNotFoundError("no such file: %s" % snr_file)
-    snrs_used = np.load(snr_file, allow_pickle=True)[0]
-    root = os.path.join(path_to_set, "wav_processed", dirry, "")
+def _read_convolved(root, i_rir, noise, nb_ch):
+    """The convolved target, noise and mixture of every microphone of RIR i_rir under wav_processed/<snr>/ (`root`),
+    as tango.py:74-109 and get_z_signals.py:75-90 read them: lists [node][ch] of float32 arrays, and their rate.
+    Every file must have the length and rate of the first: ValueError naming the file otherwise; a missing file
+    raises FileNotFoundError with its path."""
     y, s, n = ([[] for _ in nb_ch] for _ in range(3))
     fs = length = None
     ii_ch = 0
@@ -93,6 +84,23 @@ def get_input_signals(i_rir, scenario="living", noise="ssn", snr_range=None, *, 
                     raise ValueError("%s: %d samples at %d Hz, the RIR's first file has %d at %d Hz"
                                      % (path, len(x), rate, length, fs))
                 lst[i_nod].append(x)
+    return y, s, n, fs
+
+
+def get_input_signals(i_rir, scenario="living", noise="ssn", snr_range=None, *, path_to_dataset=PATH_TO_DATASET,
+                      nb_ch=(4, 4, 4, 4)):
+    """tango.py:55-111: the convolved target, noise and mixture of every microphone of RIR i_rir (lists [node][ch]
+    of float32 arrays), the dry target and noise, the sampling rate and the mixing SNR stored with the data set.
+    n_dry is scaled by that SNR in float32, as the reference's in-place `*=` on its float32 array does.
+    Every convolved file must have the length and rate of the first and the dry files its rate: ValueError naming
+    the file otherwise; a missing file raises FileNotFoundError with its path."""
+    path_to_set = os.path.join(path_to_dataset, "disco", scenario, get_dset(i_rir))
+    dirry = get_directory_name([[0, 6]] if snr_range is None else snr_range)
+    snr_file = os.path.join(path_to_set, "log", "snrs", "dry", dirry, "") + "{}_{}.npy".format(str(i_rir), noise)
+    if not os.path.isfile(snr_file):
+        raise FileNotFoundError("no such file: %s" % snr_file)
+    snrs_used = np.load(snr_file, allow_pickle=True)[0]
+    y, s, n, fs = _read_convolved(os.path.join(path_to_set, "wav_processed", dirry, ""), i_rir, noise, nb_ch)
     dry = []
     for path in (os.path.join(path_to_set, "wav_original/dry/target/") + str(i_rir) + "_S-1.wav",
                  os.path.join(path_to_set, "wav_original/dry/noise/") + str(i_rir) + "_S-2_" + noise + ".wav"):
