@@ -337,10 +337,20 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM, OUT>::THREADS, 1) stft_scm_k
         if (G::REALLOC && !G::DEAL) set_maxnreg<G::REG_LEAD, G::REG_LAUNCH>();
         if (warp != 0) return;
         // =========================================================== LOADER (+ Nyquist bin)
+        // Per tile `it`: stage tile it + NSTG - 1, then the Nyquist work of tile it.  Nothing on this chain divides by
+        // the tile count or waits for a global load: two tile cursors (the next tile to stage, the Nyquist tile) walk
+        // the range, the Nyquist masks are loaded a tile ahead and the Nyquist filter taps when the staging enters a
+        // group.  (Staging as soon as samp_empty allows instead, ahead of the Nyquist work, was slower: DESIGN.md 4.1.)
         RoleClocks rc;
-        auto load_tile = [&](int it) {
-            int grp, t0;
-            tile_of(it, grp, t0);
+        // tile cursors: (group, tile within the group) of the CTA's first tile, advanced tile by tile
+        const int grp_lo = (int)(lo / tiles_per_grp), tg_lo = (int)(lo % tiles_per_grp);
+        auto next_tile = [&](int& grp, int& tg) {
+            if (++tg == tiles_per_grp) {
+                tg = 0;
+                ++grp;
+            }
+        };
+        auto stage_tile = [&](int it, int grp, int t0) {
             const int nfr = min(TT, T - t0), s = it % NSTG, c_valid = min(C, p.n_sig - grp * C);
             rc.wait(RC_SAMP_EMPTY, &samp_empty[s], ((it / NSTG) & 1) ^ 1);
             const float* xg = p.x + (size_t)grp * C * L;
@@ -394,26 +404,63 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM, OUT>::THREADS, 1) stft_scm_k
                 for (int u = 0; u < NSLOT; ++u) as[q][u] = an[q][u] = 0.f;
         };
         nyq_reset();
-        // filter consumer: the Nyquist-bin taps of the current group, lane <-> frame
-        float2 nw1[FILT ? C : 1], nw2[FILT ? C : 1];
-        int nw_grp = -1;
-        for (int i = 0; i < NSTG - 1; ++i)
-            if (i < n_it) load_tile(i);
-        for (int it = 0; it < n_it; ++it) {
-            if (it + NSTG - 1 < n_it) load_tile(it + NSTG - 1);
-            int grp, t0;
-            tile_of(it, grp, t0);
-            const int nfr = min(TT, T - t0), s = it % NSTG, c_valid = min(C, p.n_sig - grp * C);
+        int st_grp = grp_lo, st_tg = tg_lo;       // the next tile to stage
+        int ny_grp = grp_lo, ny_tg = tg_lo;       // the Nyquist tile `it` below
+        // filter consumer: the Nyquist-bin taps of the Nyquist tile's group (nw), and those of the last staged tile's
+        // group (pw), loaded when the staging enters the group, a tile before the Nyquist work needs them; lane <-> frame
+        constexpr int NW = FILT ? C : 1;
+        float2 nw1[NW], nw2[NW], pw1[NW], pw2[NW];
+        int nw_grp = grp_lo, pw_grp = grp_lo;
+        static_assert(NSTG == 2, "a new group's Nyquist taps are those of the last staged tile");
+        auto load_taps = [&](float2 (&w1)[NW], float2 (&w2)[NW], int grp) {
             if constexpr (FILT) {
-                if (grp != nw_grp) {   // a CTA's tile range may cross groups
+#pragma unroll
+                for (int c = 0; c < C; ++c) {
+                    w1[c] = p.W1[((size_t)grp * F + F - 1) * C + c];
+                    w2[c] = p.W2[((size_t)grp * F + F - 1) * C + c];
+                }
+            }
+        };
+        auto stage_next = [&](int it) {
+            if (FILT && st_grp != pw_grp) {
+                load_taps(pw1, pw2, st_grp);
+                pw_grp = st_grp;
+            }
+            stage_tile(it, st_grp, st_tg * TT);
+            next_tile(st_grp, st_tg);
+        };
+        // pass 1: the Nyquist tile's mask values (lane <-> frame), loaded one tile ahead of their use
+        float mq[NMX];
+        auto load_masks = [&]() {
+            const int t0 = ny_tg * TT, nfr = min(TT, T - t0);
+#pragma unroll
+            for (int q = 0; q < NMX; ++q) mq[q] = (SCM && lane < nfr) ? mask_at(q, ny_grp, t0 + lane, F - 1) : 0.f;
+        };
+        for (int i = 0; i < NSTG - 1; ++i)
+            if (i < n_it) stage_next(i);
+        if constexpr (FILT)
+            load_taps(nw1, nw2, grp_lo);
+        else
+            load_masks();
+        int ny_slot = SCM ? seg_slot(grp_lo) : 0;   // the CTA's partial-sum slot of the Nyquist tile's group (0 for a later group)
+        for (int it = 0; it < n_it; ++it) {
+            const int s = it % NSTG;
+            const uint32_t ph = (it / NSTG) & 1;
+            if constexpr (FILT) {
+                if (ny_grp != nw_grp) {   // a CTA's tile range may cross groups; tile it was the last one staged
 #pragma unroll
                     for (int c = 0; c < C; ++c) {
-                        nw1[c] = p.W1[((size_t)grp * F + F - 1) * C + c];
-                        nw2[c] = p.W2[((size_t)grp * F + F - 1) * C + c];
+                        nw1[c] = pw1[c];
+                        nw2[c] = pw2[c];
                     }
-                    nw_grp = grp;
+                    nw_grp = ny_grp;
                 }
-                rc.wait(RC_SPEC_FULL, &spec_full[s], (it / NSTG) & 1);
+            }
+            if (it + NSTG - 1 < n_it) stage_next(it + NSTG - 1);
+            const int grp = ny_grp, t0 = ny_tg * TT;
+            const int nfr = min(TT, T - t0), c_valid = min(C, p.n_sig - grp * C);
+            if constexpr (FILT) {
+                rc.wait(RC_SPEC_FULL, &spec_full[s], ph);
                 if (lane < nfr) {
                     // the Nyquist spectrum is real; it goes through the complex helpers as (yv, 0), the value
                     // disco_stft stores there, so z, zn, yf match filter_dual on a stored Y bit for bit
@@ -433,10 +480,7 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM, OUT>::THREADS, 1) stft_scm_k
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&spec_empty[s]);
             } else {
-                float mq[NMX];
-#pragma unroll
-                for (int q = 0; q < NMX; ++q) mq[q] = (SCM && lane < nfr) ? mask_at(q, grp, t0 + lane, F - 1) : 0.f;
-                rc.wait(RC_SPEC_FULL, &spec_full[s], (it / NSTG) & 1);
+                rc.wait(RC_SPEC_FULL, &spec_full[s], ph);
 #pragma unroll
                 for (int r = lane; r < TT * C; r += 32) {
                     const int tl_l = r / C, c_l = r % C;
@@ -471,9 +515,9 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM, OUT>::THREADS, 1) stft_scm_k
                             }
                         }
                     }
-                    const bool seg_end = (it + 1 == n_it) || ((lo + it + 1) % tiles_per_grp == 0);
+                    const bool seg_end = (it + 1 == n_it) || (ny_tg + 1 == tiles_per_grp);
                     if (seg_end) {
-                        float* out = p.part + ((size_t)grp * p.slots_per_grp + seg_slot(grp)) * NACC * F + (F - 1);
+                        float* out = p.part + ((size_t)grp * p.slots_per_grp + ny_slot) * NACC * F + (F - 1);
 #pragma unroll
                         for (int u = 0; u < NSLOT; ++u) {
                             const int pp = lane + 32 * u;
@@ -492,11 +536,16 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM, OUT>::THREADS, 1) stft_scm_k
                             }
                         }
                         nyq_reset();
+                        ny_slot = 0;   // this CTA holds the first tile of every later group in its range
                     }
                 }
                 __syncwarp();   // nyq[] is rewritten by the next tile
             }
             rc.tile();
+            next_tile(ny_grp, ny_tg);
+            if constexpr (!FILT) {
+                if (it + 1 < n_it) load_masks();
+            }
         }
         rc.done(RC_ROLE_LOADER);
     } else if (is_fft) {
