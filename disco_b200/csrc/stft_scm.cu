@@ -320,6 +320,15 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM, OUT>::THREADS, 1) stft_scm_k
         grp = (int)(i / tiles_per_grp);
         t0 = (int)(i % tiles_per_grp) * TT;
     };
+    // The loader and the consumer warps walk their tiles with a cursor, (group, tile within the group), that starts
+    // at the range's first tile (grp_lo, tg_lo) and advances tile by tile, so that no tile costs them a 64-bit
+    // division (but the 1024-point SCM consumers, below).  The FFT warps still divide once per tile, in enter_tile.
+    auto next_tile = [&](int& grp, int& tg) {
+        if (++tg == tiles_per_grp) {
+            tg = 0;
+            ++grp;
+        }
+    };
     auto seg_slot = [&](int grp) { return blockIdx.x - seg_slots(grp, tiles_per_grp, total, gridDim.x).first; };
     auto mask_at = [&](int q, int grp, int t, int f) {
         const float* m = q == 0 ? p.mask : p.mask2;
@@ -342,14 +351,7 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM, OUT>::THREADS, 1) stft_scm_k
         // the range, the Nyquist masks are loaded a tile ahead and the Nyquist filter taps when the staging enters a
         // group.  (Staging as soon as samp_empty allows instead, ahead of the Nyquist work, was slower: DESIGN.md 4.1.)
         RoleClocks rc;
-        // tile cursors: (group, tile within the group) of the CTA's first tile, advanced tile by tile
         const int grp_lo = (int)(lo / tiles_per_grp), tg_lo = (int)(lo % tiles_per_grp);
-        auto next_tile = [&](int& grp, int& tg) {
-            if (++tg == tiles_per_grp) {
-                tg = 0;
-                ++grp;
-            }
-        };
         auto stage_tile = [&](int it, int grp, int t0) {
             const int nfr = min(TT, T - t0), s = it % NSTG, c_valid = min(C, p.n_sig - grp * C);
             rc.wait(RC_SAMP_EMPTY, &samp_empty[s], ((it / NSTG) & 1) ^ 1);
@@ -688,10 +690,9 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM, OUT>::THREADS, 1) stft_scm_k
         if constexpr (FILT) {
             // =========================================================== filter consumer: thread <-> bin f
             float2 w1[C], w2[C];
-            int w_grp = -1;
-            for (int it = 0; it < n_it; ++it) {
-                int grp, t0;
-                tile_of(it, grp, t0);
+            int w_grp = -1, grp = (int)(lo / tiles_per_grp), tg = (int)(lo % tiles_per_grp);
+            for (int it = 0; it < n_it; ++it, next_tile(grp, tg)) {
+                const int t0 = tg * TT;
                 const int nfr = min(TT, T - t0), s = it % NSTG;
                 if (grp != w_grp) {   // a CTA's tile range may cross groups
 #pragma unroll
@@ -775,15 +776,30 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM, OUT>::THREADS, 1) stft_scm_k
         }
         ScmAcc<C, NM> acc;
         float mk[NMX][MC];
-        // masks of chunk `ch` of tile `it` (a chunk past the CTA's last tile loads nothing): one base pointer per
-        // mask, frame stride hoisted (frame-major: F floats, (F, T) layout: 1)
+        // masks of chunk `ch` of the tile at frame t0 of group grp: one base pointer per mask, frame stride hoisted
+        // (frame-major: F floats, (F, T) layout: 1).  A chunk whose frames all exist (every chunk but the last of a
+        // group's last tile) loads with compile-time offsets and no per-frame bounds test.  That second copy of the
+        // loads is kept to the variants of at most 512 points and 4 microphones, whose consumer warps have registers
+        // to spare; the others load as before.
+        constexpr bool MFAST = !G::WIDE && N <= 512;
         const int m_st = p.mask_ft ? 1 : F;
         const size_t m_f = p.mask_ft ? (size_t)f * T : (size_t)f;
-        auto load_mask = [&](int it, int ch) {
-            if (it >= n_it) return;
-            int grp, t0;
-            tile_of(it, grp, t0);
+        auto load_mask = [&](int grp, int t0, int ch) {
             const size_t base = (size_t)grp * T * F + m_f + (size_t)(t0 + ch * MC) * m_st;
+            if (MFAST && (ch + 1) * MC <= TT && t0 + (ch + 1) * MC <= T) {
+#pragma unroll
+                for (int q = 0; q < NM; ++q) {
+                    const float* mb = (q == 0 ? p.mask : p.mask2) + base;
+                    if (p.mask_ft) {
+#pragma unroll
+                        for (int i = 0; i < MC; ++i) mk[q][i] = mb[i];
+                    } else {
+#pragma unroll
+                        for (int i = 0; i < MC; ++i) mk[q][i] = mb[i * F];
+                    }
+                }
+                return;
+            }
 #pragma unroll
             for (int q = 0; q < NM; ++q) {
                 const float* mb = (q == 0 ? p.mask : p.mask2) + base;
@@ -792,13 +808,20 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM, OUT>::THREADS, 1) stft_scm_k
                     mk[q][i] = (ch * MC + i < TT && t0 + ch * MC + i < T) ? mb[i * m_st] : 0.f;
             }
         };
+        int grp = (int)(lo / tiles_per_grp), tg = (int)(lo % tiles_per_grp);
         if (SCM) {
             acc.reset();
-            load_mask(0, 0);
+            load_mask(grp, tg * TT, 0);
         }
+        // The 1024-point variants, whose FFT warps spill already, keep locating each tile by division: the cursor held
+        // across their tile loop costs them spill traffic.
+        constexpr bool CURSOR = N <= 512;
         for (int it = 0; it < n_it; ++it) {
-            int grp, t0;
-            tile_of(it, grp, t0);
+            if constexpr (!CURSOR) {
+                grp = (int)((lo + it) / tiles_per_grp);
+                tg = (int)((lo + it) % tiles_per_grp);
+            }
+            const int t0 = tg * TT;
             const int nfr = min(TT, T - t0), s = it % NSTG, c_valid = min(C, p.n_sig - grp * C);
             const float2* stage = spec + s * G::SPEC;
             float2* ybase = p.Y + ((size_t)grp * C * T + t0) * F + f;
@@ -811,11 +834,11 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM, OUT>::THREADS, 1) stft_scm_k
                 for (int q = 0; q < NMX; ++q)
 #pragma unroll
                     for (int i = 0; i < MC; ++i) mcur[q][i] = SCM ? mk[q][i] : 0.f;
-                if (SCM) {   // next chunk's masks: in flight while this chunk is processed
+                if (SCM) {   // next chunk's masks (none past the CTA's last tile): in flight while this chunk is processed
                     if (ch + 1 < NCH)
-                        load_mask(it, ch + 1);
-                    else
-                        load_mask(it + 1, 0);
+                        load_mask(grp, t0, ch + 1);
+                    else if (it + 1 < n_it)
+                        load_mask(tg + 1 < tiles_per_grp ? grp : grp + 1, tg + 1 < tiles_per_grp ? (tg + 1) * TT : 0, 0);
                 }
                 if (ch == 0) rc.wait(RC_SPEC_FULL, &spec_full[s], (it / NSTG) & 1);
 #pragma unroll
@@ -848,12 +871,13 @@ __global__ void __launch_bounds__(StftCfg<N, C, NM, OUT>::THREADS, 1) stft_scm_k
             }
             __syncwarp();
             if (lane == 0) mbar_arrive(&spec_empty[s]);
-            const bool seg_end = (it + 1 == n_it) || ((lo + it + 1) % tiles_per_grp == 0);
+            const bool seg_end = (it + 1 == n_it) || (tg + 1 == tiles_per_grp);
             if (SCM && seg_end) {
                 acc.flush(p.part + ((size_t)grp * p.slots_per_grp + seg_slot(grp)) * NACC * F + f, F);
                 acc.reset();
             }
             rc.tile();
+            next_tile(grp, tg);
         }
         rc.done(RC_ROLE_SCM);
     }
