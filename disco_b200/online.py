@@ -12,8 +12,8 @@ utterances, nodes, bins and blocks (csrc/online.cu + the batched solver):
     mwf_solve          one GEVD-MWF per (block, bin)
     filter_sum_blocks  frame t filtered with the filter of block t // block - lag
 
-Every channel stack up to D = 16 runs, the MEETIT geometry (8 nodes x 2 mics, step 2 at D = 9) included;
-the chunked `stream.OnlineTangoStream` covers D <= 8.
+Every channel stack up to D = 16 runs, the MEETIT geometry (8 nodes x 2 mics, step 2 at D = 9) included, in
+the whole-signal call and in the chunked `stream.OnlineTangoStream` alike (D >= 9 there with wide=True).
 
 `lag = 1` is strictly causal with an algorithmic delay of 0 frames (the filter in force was finished before
 the frame arrived); `lag = 0` uses the block's own statistics (look-ahead of up to block - 1 frames).
