@@ -1,5 +1,6 @@
 // C ABI of libdisco_b200.so (declared in include/disco_b200.h): argument checking, per-device
 // constant tables, launch-geometry choices.  No torch types cross this boundary.
+#include <limits.h>
 #include <math.h>
 #include <stdlib.h>
 #include <stdio.h>
@@ -50,6 +51,15 @@ int cuda_fail(cudaError_t e, const char* where) {
     } while (0)
 
 bool valid_nfft(int n) { return n == 256 || n == 512 || n == 1024; }
+
+// The longest whole signal, and the largest sample position of a stream record, that the STFT / iSTFT kernels address
+// in int: they form positions up to a frame and a CTA stride (together < 1024 + n_fft samples) past the signal's end
+long long max_length(int n_fft) { return (long long)INT_MAX - n_fft - 1024; }
+bool too_long(int length, int n_fft) {
+    if (length <= max_length(n_fft)) return false;
+    fail(DISCO_ERR_INVALID, "length past 2^31 - 1 - n_fft - 1024 samples");
+    return true;
+}
 
 struct Tables {
     float2* twiddle = nullptr;   // [N/32][32] W_N^(l k1)
@@ -128,6 +138,7 @@ int stft_common(const float* x, const float* mask, const float* mask2, int mask_
     if (!valid_nfft(n_fft)) return fail(DISCO_ERR_INVALID, "n_fft must be 256, 512 or 1024");
     if (n_sig <= 0 || length <= n_fft / 2)
         return fail(DISCO_ERR_INVALID, "need n_sig > 0 and length > n_fft/2 (reflect padding)");
+    if (too_long(length, n_fft)) return DISCO_ERR_INVALID;
     if (C < 1) return fail(DISCO_ERR_INVALID, "C must be positive");
     if (!stft_scm_supported(n_fft, C, n_mask))
         return fail(DISCO_ERR_UNSUPPORTED,
@@ -226,6 +237,7 @@ int disco_stft_filter_dual(const float* x, const void* W1, const void* W2, void*
     if (!valid_nfft(n_fft)) return fail(DISCO_ERR_INVALID, "n_fft must be 256, 512 or 1024");
     if (n_grp < 1 || length <= n_fft / 2)
         return fail(DISCO_ERR_INVALID, "need n_grp > 0 and length > n_fft/2 (reflect padding)");
+    if (too_long(length, n_fft)) return DISCO_ERR_INVALID;
     if (!stft_scm_supported(n_fft, C, 2))
         return fail(DISCO_ERR_UNSUPPORTED, "fused STFT+filter: 1..4 channels per group, n_fft 256 or 512");
     if (ref < 0 || ref >= C) return fail(DISCO_ERR_INVALID, "ref channel out of range");
@@ -485,6 +497,7 @@ int disco_filter_dual(const void* W1, const void* W2, const void* Y, void* z, vo
 int disco_istft(const void* Y, float* x, int n_sig, int T, int length, int n_fft, void* stream) {
     if (!valid_nfft(n_fft)) return fail(DISCO_ERR_INVALID, "n_fft must be 256, 512 or 1024");
     if (n_sig <= 0 || T < 1 || length < 1 || !Y || !x) return fail(DISCO_ERR_INVALID, "bad arguments");
+    if (too_long(length, n_fft)) return DISCO_ERR_INVALID;
     Tables tb;
     int rc = get_tables(n_fft, &tb);
     if (rc) return rc;
@@ -518,6 +531,7 @@ int disco_stft_lengths(const float* x, const int* lengths, const int* lengths_ho
     if (!valid_nfft(n_fft)) return fail(DISCO_ERR_INVALID, "n_fft must be 256, 512 or 1024");
     if (n_sig <= 0 || length <= n_fft / 2)
         return fail(DISCO_ERR_INVALID, "need n_sig > 0 and length > n_fft/2 (reflect padding)");
+    if (too_long(length, n_fft)) return DISCO_ERR_INVALID;
     int rc = check_lengths(lengths_host, n_sig, n_fft / 2, length);
     if (rc) return rc;
     if (!x || !lengths || !Y) return fail(DISCO_ERR_INVALID, "null pointer");
@@ -542,6 +556,7 @@ int disco_istft_lengths(const void* Y, const int* lengths, const int* lengths_ho
                         int length, int n_fft, void* stream) {
     if (!valid_nfft(n_fft)) return fail(DISCO_ERR_INVALID, "n_fft must be 256, 512 or 1024");
     if (n_sig <= 0 || T < 1 || length < 1) return fail(DISCO_ERR_INVALID, "bad arguments");
+    if (too_long(length, n_fft)) return DISCO_ERR_INVALID;
     int rc = check_lengths(lengths_host, n_sig, 0, length);
     if (rc) return rc;
     if (!Y || !lengths || !x) return fail(DISCO_ERR_INVALID, "null pointer");
@@ -667,23 +682,31 @@ int disco_filter_sum_blocks_lengths(const void* W, int conj_w, const void* Y, co
                                     n_sel, frames, frames_host, stream);
 }
 
+// Stream records hold positions relative to an origin of the caller's choice (a multiple of the hop, 0 at the stream's
+// start), so only their distances matter; every position a kernel forms from an accepted record stays below
+// max_length(n_fft).  The checks run in 64 bits, so no field of a record can wrap them.
+//
 // A stream STFT record against the buffers it addresses: chunk rows of n_max samples, f_max frame rows of Y, and
 // (Y_blk) blk_frames rows of the block buffer
 static int check_stft_record(const StftSlot& r, int n_fft, int n_max, int f_max, int blk_frames, const void* chunk,
                              const void* Y, const void* Y_blk) {
+    typedef long long i64;
     if (r.n_new < 0 || r.n_new > n_max || r.length < r.n_new || r.t0 < 0 || r.n_fr < 0 || r.n_fr > f_max ||
         (r.hist_sel != 0 && r.hist_sel != 1))
         return fail(DISCO_ERR_INVALID, "bad sizes");
+    const i64 H = n_fft / 2;
+    if (r.length > max_length(n_fft) || ((i64)r.t0 + r.n_fr) * H > max_length(n_fft))
+        return fail(DISCO_ERR_INVALID, "positions past 2^31 - 1 - n_fft - 1024 samples: rebase the record");
     if ((r.n_new > 0 && !chunk) || (r.n_fr > 0 && !Y) || (r.final_call && r.n_new > 0))
         return fail(DISCO_ERR_INVALID, "null pointer (or a chunk on the final call)");
     if (r.n_fr > 0) {
         // every sample the frames read has arrived (the last frame is reflected at the end on the final call), and
         // the first one lies within the carried history
-        const int H = n_fft / 2, L0 = r.length - r.n_new, t1 = r.t0 + r.n_fr - 1;
+        const i64 L0 = (i64)r.length - r.n_new, t1 = (i64)r.t0 + r.n_fr - 1;
         const bool arrived = r.length > H && (r.final_call ? t1 <= r.length / H : (t1 == 0 || (t1 + 1) * H <= r.length));
         if (!arrived || (r.t0 >= 1 && (r.t0 - 1) * H < L0 - n_fft))
             return fail(DISCO_ERR_INVALID, "frames not complete, or older than the carried history");
-        if (Y_blk && (r.blk_slot < 0 || r.blk_slot + r.n_fr > blk_frames))
+        if (Y_blk && (r.blk_slot < 0 || (i64)r.blk_slot + r.n_fr > blk_frames))
             return fail(DISCO_ERR_INVALID, "frames outside the block buffer");
     }
     return 0;
@@ -691,18 +714,22 @@ static int check_stft_record(const StftSlot& r, int n_fft, int n_max, int f_max,
 
 // A stream iSTFT record against the buffers it addresses: f_max frame rows of Y and rows of s_max samples of x
 static int check_istft_record(const IstftSlot& r, int n_fft, int f_max, int s_max, const void* Y, const float* x) {
+    typedef long long i64;
     if (r.t0 < 0 || r.n_fr < 0 || r.n_fr > f_max || r.x_first < 0 || (r.length < 1 && (r.n_fr > 0 || r.final_call)))
         return fail(DISCO_ERR_INVALID, "bad sizes");
+    const i64 H = n_fft / 2;
+    if (r.length > max_length(n_fft) || r.x_first > max_length(n_fft) ||
+        ((i64)r.t0 + r.n_fr) * H > max_length(n_fft))
+        return fail(DISCO_ERR_INVALID, "positions past 2^31 - 1 - n_fft - 1024 samples: rebase the record");
     if (r.n_fr > 0 && !Y) return fail(DISCO_ERR_INVALID, "null pointer");
     if (r.n_fr <= 0 && !r.final_call) return 0;   // not run
     // samples written: the hop blocks max(t0, 1) .. t0 + n_fr - 1, and on the final call the rest up to length
-    const int H = n_fft / 2;
-    const int lo = (r.t0 > 0 ? r.t0 - 1 : 0) * H;
-    int hi = r.final_call ? r.length : (r.t0 + r.n_fr - 1) * H;
+    const i64 lo = (r.t0 > 0 ? r.t0 - 1 : 0) * H;
+    i64 hi = r.final_call ? r.length : ((i64)r.t0 + r.n_fr - 1) * H;
     if (hi > r.length) hi = r.length;
     if (hi > lo) {
         if (!x) return fail(DISCO_ERR_INVALID, "null pointer");
-        if (lo < r.x_first || hi > r.x_first + s_max) return fail(DISCO_ERR_INVALID, "output samples outside x");
+        if (lo < r.x_first || hi > (i64)r.x_first + s_max) return fail(DISCO_ERR_INVALID, "output samples outside x");
     }
     return 0;
 }

@@ -59,10 +59,11 @@ DISCO_DEV void stft_unmix(float2 zf, float2 zn, float2& a, float2& b) {
 DISCO_DEV float stft_nyquist(float2 z, bool second) { return second ? z.y + z.y : z.x + z.x; }
 
 // Sample index s of the padded signal of length L: librosa center=True, pad_mode='reflect' (an index still outside
-// [0, L) afterwards, possible only for L <= N/2, reads as zero at the caller)
+// [0, L) afterwards, possible only for L <= N/2, reads as zero at the caller).  The end is mirrored as (L - 1) -
+// (s - (L - 1)), not 2 (L - 1) - s, which would overflow int for L > 2^30 + 1.
 DISCO_DEV int reflect_index(int s, int L) {
     if (s < 0) s = -s;
-    if (s >= L) s = 2 * (L - 1) - s;
+    if (s >= L) s = (L - 1) - (s - (L - 1));
     return s;
 }
 

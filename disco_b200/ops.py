@@ -640,10 +640,13 @@ def stream_stft(hist, chunk, length, t0, n_fr, n_fft=512, hist_out=None, Y_blk=N
         P = Y_blk.shape[-2]
         if tuple(Y_blk.shape) != lead + (P, F):
             raise ValueError("Y_blk shape %s, expected %s" % (tuple(Y_blk.shape), lead + (P, F)))
+    n_sig, n_new, P = _c_int(n_sig, "n_sig"), _c_int(chunk.shape[-1], "chunk length"), _c_int(P, "Y_blk frames")
+    r = _records(_scalar_record((length, n_new, t0, n_fr, blk_slot, 1 if final else 0, 0, 0)), 1, STFT_SLOT_FIELDS,
+                 "record", n_fft)[0]
     Y = torch.empty(lead + (int(n_fr), F), dtype=torch.complex64, device=hist.device)
     _lib.check(_lib.load().disco_stream_stft(_ptr(hist), _ptr(chunk) if chunk.numel() else None, _ptr(hist_out),
-                                             _ptr(Y), _ptr(Y_blk), n_sig, chunk.shape[-1], int(length), int(t0),
-                                             int(n_fr), P, int(blk_slot), 1 if final else 0, n_fft, _stream()))
+                                             _ptr(Y), _ptr(Y_blk), n_sig, n_new, int(r[0]), int(r[2]), int(r[3]), P,
+                                             int(r[4]), int(r[5]), n_fft, _stream()))
     return Y
 
 
@@ -665,31 +668,97 @@ def stream_istft(Y, carry, t0, length, n_fft=512, final=False, x=None, x_first=0
     lo = max(int(t0) - 1, 0) * H
     hi = min(int(length), int(length) if final else (int(t0) + n_fr - 1) * H)
     if x is None:
-        x = torch.empty(lead + (max(hi - lo, 0),), dtype=torch.float32, device=Y.device)
         x_first = lo
     else:
         _need(x, torch.float32, "x")
         if tuple(x.shape[:-1]) != lead:
             raise ValueError("x shape %s, expected %s" % (tuple(x.shape), lead + (-1,)))
+    n_sig = _c_int(n_sig, "n_sig")
+    s_max = _c_int(max(hi - lo, 0) if x is None else x.shape[-1], "x length")
+    r = _records(_scalar_record((t0, n_fr, length, 1 if final else 0, x_first)), 1, ISTFT_SLOT_FIELDS, "record",
+                 n_fft)[0]
+    if x is None:
+        x = torch.empty(lead + (s_max,), dtype=torch.float32, device=Y.device)
     _lib.check(_lib.load().disco_stream_istft(_ptr(Y) if Y.numel() else None, _ptr(carry), _ptr(x) if x.numel() else None,
-                                              n_sig, int(t0), int(n_fr), int(length), 1 if final else 0, int(x_first),
-                                              x.shape[-1], n_fft, _stream()))
+                                              n_sig, int(r[0]), int(r[1]), int(r[2]), int(r[3]), int(r[4]), s_max,
+                                              n_fft, _stream()))
     return x
 
 
 STFT_SLOT_FIELDS = ("length", "n_new", "t0", "n_fr", "blk_slot", "final", "hist_sel", "hist_write")
 ISTFT_SLOT_FIELDS = ("t0", "n_fr", "length", "final", "x_first")
+INT_MAX = 2 ** 31 - 1
 
 
-def _records(slots, n_slot, fields, name):
-    """Per-slot records [n_slot, len(fields)] as a contiguous host int32 array."""
+def max_stream_length(n_fft=512):
+    """The largest sample position of a stream record the library accepts, relative to the record's origin, and the
+    longest whole signal its STFT / iSTFT take: the kernels form positions up to a frame and a CTA stride past it in
+    C int.  The stream ops rebase their records (_rebase), so a stream itself may run without an end."""
+    return INT_MAX - n_fft - 1024
+
+
+def _c_int(v, name):
+    v = int(v)
+    if not -INT_MAX - 1 <= v <= INT_MAX:
+        raise ValueError("%s = %d does not fit in a C int" % (name, v))
+    return v
+
+
+def _scalar_record(values):
+    """One record [1, n] of host integers of any size (ValueError past int64)."""
+    try:
+        return np.array([[int(v) for v in values]], dtype=np.int64)
+    except OverflowError:
+        raise ValueError("a stream position does not fit in 64 bits: %s" % (values,)) from None
+
+
+def _rebase(rec, fields, n_fft):
+    """Absolute stream records [n_slot, len(fields)] (int64) relative to an origin O per slot.
+
+    O is a multiple of the hop H; it lies at or before every sample the call reads, writes or carries: the history
+    start length - n_new - n_fft and the first sample (t0 - 1) H of frame t0 (STFT); the first sample (t0 - 1) H of
+    hop block t0, x_first and length - 1 (iSTFT).  O = 0 whenever the call can reach the start reflection (t0 = 0, or
+    fewer than n_fft samples before the chunk).  length and x_first lose O, t0 loses O / H.  The kernels use positions
+    only to address the history, the chunk and x and to place the two reflections, so a call's outputs do not depend
+    on O, and a valid record stays valid.  Formed without a product, so no int64 position overflows."""
+    H = n_fft // 2
+    rec = rec.copy()
+    if H < 1:                 # no such transform: the library rejects the call
+        return rec
+    if fields is STFT_SLOT_FIELDS:
+        length, n_new, t0 = rec[:, 0], rec[:, 1], rec[:, 2]
+        o = np.maximum(np.minimum((length - n_new - n_fft) // H, t0 - 1), 0)
+        rec[:, 0] -= o * H
+        rec[:, 2] -= o
+    else:
+        t0, length, x_first = rec[:, 0], rec[:, 2], rec[:, 4]
+        o = np.maximum(np.minimum(np.minimum(t0 - 1, x_first // H), (length - 1) // H), 0)
+        rec[:, 0] -= o
+        rec[:, 2] -= o * H
+        rec[:, 4] -= o * H
+    return rec
+
+
+def _records(slots, n_slot, fields, name, n_fft):
+    """Per-slot records [n_slot, len(fields)] of absolute positions, rebased (_rebase), as a contiguous host int32
+    array.  ValueError for a field that does not fit in a C int after rebasing: nothing is narrowed silently."""
     arr = np.asarray(slots)
+    if arr.dtype.kind == "O" and arr.size and all(isinstance(v, int) for v in arr.ravel()):
+        raise ValueError("%s: a position does not fit in 64 bits" % name)
     if arr.dtype.kind not in "iu":
         raise TypeError("%s must be integers, got %s" % (name, arr.dtype))
     if tuple(arr.shape) != (n_slot, len(fields)):
         raise ValueError("%s shape %s, expected (%d, %d): %s" % (name, tuple(arr.shape), n_slot, len(fields),
                                                                 ", ".join(fields)))
-    return np.ascontiguousarray(arr, dtype=np.int32)
+    if arr.dtype.kind == "u" and arr.size and arr.max() > np.iinfo(np.int64).max:
+        raise ValueError("%s: a position does not fit in 64 bits" % name)
+    rec = _rebase(arr.astype(np.int64), fields, n_fft)
+    bad = (rec < -INT_MAX - 1) | (rec > INT_MAX)
+    if bad.any():
+        s, f = np.argwhere(bad)[0]
+        raise ValueError("%s: slot %d's %s = %d does not fit in a C int, even relative to the stream's origin"
+                         % (name, s, fields[f], rec[s, f]))
+    return np.ascontiguousarray(rec, dtype=np.int32)
 
 
 @_on_device
@@ -714,13 +783,15 @@ def stream_stft_slots(hist, chunk, slots, f_max, n_fft=512, Y_blk=None):
         P = Y_blk.shape[-2]
         if tuple(Y_blk.shape) != lead + (P, F):
             raise ValueError("Y_blk shape %s, expected %s" % (tuple(Y_blk.shape), lead + (P, F)))
-    host = _records(slots, S, STFT_SLOT_FIELDS, "slots")
-    Y = torch.empty(lead + (int(f_max), F), dtype=torch.complex64, device=hist.device)
+    host = _records(slots, S, STFT_SLOT_FIELDS, "slots", n_fft)
+    n_sig, n_max = _c_int(n_sig, "n_sig"), _c_int(chunk.shape[-1], "chunk length")
+    f_max, P = _c_int(f_max, "f_max"), _c_int(P, "Y_blk frames")
+    Y = torch.empty(lead + (f_max, F), dtype=torch.complex64, device=hist.device)
     dev = torch.from_numpy(host).to(hist.device)
     _lib.check(_lib.load().disco_stream_stft_slots(_ptr(hist), _ptr(chunk) if chunk.numel() else None,
                                                    _ptr(Y) if Y.numel() else None, _ptr(Y_blk), _ptr(dev),
-                                                   host.ctypes.data_as(_lib.c_int_p), S, n_sig, chunk.shape[-1],
-                                                   int(f_max), P, n_fft, _stream()))
+                                                   host.ctypes.data_as(_lib.c_int_p), S, n_sig, n_max, f_max, P, n_fft,
+                                                   _stream()))
     return Y
 
 
@@ -741,12 +812,13 @@ def stream_istft_slots(Y, carry, slots, x, n_fft=512):
                          % (tuple(Y.shape), tuple(carry.shape), tuple(x.shape), H + 1, H))
     S = lead[0]
     n_sig = int(np.prod(lead[1:], dtype=np.int64))
-    host = _records(slots, S, ISTFT_SLOT_FIELDS, "slots")
+    host = _records(slots, S, ISTFT_SLOT_FIELDS, "slots", n_fft)
+    n_sig, f_max, s_max = _c_int(n_sig, "n_sig"), _c_int(f_max, "f_max"), _c_int(x.shape[-1], "x length")
     dev = torch.from_numpy(host).to(Y.device)
     _lib.check(_lib.load().disco_stream_istft_slots(_ptr(Y) if Y.numel() else None, _ptr(carry),
                                                     _ptr(x) if x.numel() else None, _ptr(dev),
-                                                    host.ctypes.data_as(_lib.c_int_p), S, n_sig, f_max, x.shape[-1],
-                                                    n_fft, _stream()))
+                                                    host.ctypes.data_as(_lib.c_int_p), S, n_sig, f_max, s_max, n_fft,
+                                                    _stream()))
     return x
 
 

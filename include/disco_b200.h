@@ -307,7 +307,14 @@ DISCO_API int disco_filter_sum_blocks_lengths(const void* W, int conj_w, const v
  * disco_stream_istft turns frames [t0, t0 + n_fr) of n_sig spectra Y [n_sig][n_fr][F] into the hop blocks that
  * become final with them: samples [(max(t0, 1) - 1) hop, (t0 + n_fr - 1) hop), written to x[s - x_first] of rows
  * x_stride floats apart.  carry [n_sig][n_fft / 2] float32 holds the windowed second half of the previous frame
- * (zeros before frame 0) and is updated in place.  final_call = 1 also writes the rest of the signal up to `length`. */
+ * (zeros before frame 0) and is updated in place.  final_call = 1 also writes the rest of the signal up to `length`.
+ * Positions (length, t0, x_first) are relative to an origin the caller may choose per call: a multiple of the hop,
+ * at or before every sample the call reads, writes or carries, and 0 at the stream's start (while frame 0 or the
+ * start reflection is reachable).  Only distances from the origin reach the kernels, so the results do not depend on
+ * it, and a stream may run past 2^31 samples.  Positions must stay below the stream bound:
+ * length <= 2^31 - 1 - n_fft - 1024, (t0 + n_fr) hop and x_first likewise; a record past it is DISCO_ERR_INVALID.
+ * The same bound caps `length` of disco_stft, disco_stft_scm(2), disco_stft_filter_dual, disco_istft and their
+ * _lengths twins. */
 DISCO_API int disco_stream_stft(const float* hist, const float* chunk, float* hist_out, void* Y, void* Y_blk,
                                 int n_sig, int n_new, int length, int t0, int n_fr, int blk_frames, int blk_slot,
                                 int final_call, int n_fft, void* stream);
