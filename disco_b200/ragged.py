@@ -29,7 +29,8 @@ MAX_CHANNELS = 16          # the step-2 kernels take C + K - 1 <= 16 channels (a
 
 
 class _Layout:
-    """The packed layout of `channels`: K, the offsets, and the nodes of each channel count (ascending counts)."""
+    """The packed layout of `channels`: K, the offsets, and the nodes of each channel count (ascending counts).  M:
+    the packed rows the caller holds, or None where no rows are at hand yet (a stream, before its first chunk)."""
 
     def __init__(self, channels, M, ref_mic):
         if isinstance(channels, (str, bytes, torch.Tensor)) or not hasattr(channels, "__len__") or len(channels) == 0:
@@ -41,7 +42,7 @@ class _Layout:
                 raise ValueError("every node needs at least one microphone, got %r" % (channels,))
         self.channels = [int(c) for c in channels]
         self.K = len(self.channels)
-        if sum(self.channels) != M:
+        if M is not None and sum(self.channels) != M:
             raise ValueError("channels %r sum to %d, y holds %d rows" % (self.channels, sum(self.channels), M))
         if self.K > MAX_CHANNELS:
             raise NotImplementedError("at most %d nodes, got %d" % (MAX_CHANNELS, self.K))

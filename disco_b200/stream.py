@@ -20,12 +20,20 @@ Per push, for every run of newly completed frames (a run never crosses a block b
                          tf_mask first for the exchange modes other than 'local'),
     mwf_solve            and the block's filters W1_j, W2_j
     stream_istft         the hop blocks of yf (with clean components: of the six time signals) that became final
+
+Ragged arrays.  C may also be a sequence of K per-node microphone counts (`channels`); the inputs are then packed as
+ragged.py packs them, [B, M, n] with M = sum(channels) and node k on rows off_k .. off_k + C_k - 1.  The nodes of
+one count form a group, and every per-node stage above runs once per group on [B, n_C, C, ...]: the STFT of each
+group from its own history (so signals pair inside the group, as online_tango_ragged's per-group transforms pair
+them), step 1, step 2 with the z of all K nodes and the group's node_sel, and the block statistics and solves.  The
+buffers that span all K nodes (masks, z, outputs) are assembled with index_copy.  An int C is the one-group case.
 """
 import numpy as np
 import torch
 
 from . import ops
-from .tango import _ORACLE_SIGS, _clean_masks, _mask_kind, _ref_plane, _z_for_stats
+from .ragged import _Layout, _group_R0
+from .tango import _ORACLE_SIGS, _mask_kind, _ref_plane, _step1_mask, _step2_mask, _z_for_stats
 
 N_FFTS = (256, 512, 1024)
 # the time signals of a stream with clean components, in post.to_time's order (their iSTFT pairs signals across them)
@@ -97,15 +105,16 @@ def _check_options(filter_type, rank, mask_for_z, clean, vads):
             raise ValueError("network masks ('crnn' / 'rnn') come in through mask_fn")
 
 
-def _split_scans(Xs, Xn, Zs, Zn, mask, lambda_cor, block, R0, n_fft, frames=None):
+def _split_scans(Xs, Xn, Zs, Zn, mask, lambda_cor, block, R0, n_fft, frames=None, node_sel=None):
     """The statistics of online._online_mwf_split on a run of blocks: R_ss the unweighted recursive scan of [Xs ; Zs],
     R_nn that of [Xn ; Zn] (Xs, Xn first scaled by mask and 1 - mask when a mask is given), seeded by R0 = (R_ss,
-    R_nn) of the block before, or None.  Returns (R_ss, R_nn) [B, K, J, F, D, D]."""
+    R_nn) of the block before, or None; node_sel: the nodes Xs holds when Zs spans more.  Returns (R_ss, R_nn)
+    [B, K, J, F, D, D]."""
     if mask is not None:
         Xs, Xn = ops.apply_mask(Xs, mask, False), ops.apply_mask(Xn, mask, True)
     r0s, r0n = (None, None) if R0 is None else ((R0[0], R0[0]), (R0[1], R0[1]))   # the second matrix is not used
-    Rss, _ = ops.scm_recursive(Xs, None, Zs, lambda_cor, block, 2, r0s, n_fft, frames=frames)
-    Rnn, _ = ops.scm_recursive(Xn, None, Zn, lambda_cor, block, 2, r0n, n_fft, frames=frames)
+    Rss, _ = ops.scm_recursive(Xs, None, Zs, lambda_cor, block, 2, r0s, n_fft, node_sel=node_sel, frames=frames)
+    Rnn, _ = ops.scm_recursive(Xn, None, Zn, lambda_cor, block, 2, r0n, n_fft, node_sel=node_sel, frames=frames)
     return Rss, Rnn
 
 
@@ -134,7 +143,154 @@ def _check_masks(masks, want, device):
             raise ValueError("%s must be float32 on %s" % (name, device))
     return mz, mw
 
-class OnlineTangoStream:
+
+def _is_ragged(C):
+    """C given as per-node microphone counts (a sequence) rather than one count for every node."""
+    if isinstance(C, (str, bytes)):
+        return False
+    if isinstance(C, (torch.Tensor, np.ndarray)):
+        return C.ndim > 0
+    return hasattr(C, "__len__")
+
+
+class _Group:
+    """The nodes of one microphone count C (all K nodes when C is an int), and the state a stream or pool keeps for
+    them.  sel is the node_sel of its step-2 launches: None when the group holds every node.  Its device indices
+    are built on first use (a pool touches the device on its first open only)."""
+
+    def __init__(self, C, nodes, K, lay, device):
+        self.C, self.nodes, self.n, self.D = C, list(nodes), len(nodes), C + K - 1
+        self.sel = None if self.n == K else self.nodes
+        self._lay, self._device = lay, device
+
+    @property
+    def idx(self):
+        """The group's nodes as a device index."""
+        return self._lay.node_index(self.C, self._device)
+
+    @property
+    def rows(self):
+        """The group's packed rows as a device index, node-major."""
+        return self._lay.rows(self.C, self._device)
+
+
+class _Geometry:
+    """The channel layout of a stream or a pool: C an int (K nodes x C microphones, inputs [B, K, C, n]) or a sequence
+    of K counts (channels: the packed inputs [B, M, n] of ragged.py).  Either way the nodes of one count form a
+    group, and the per-node stages run once per group; these helpers move tensors between the groups and the
+    layouts that span all K nodes."""
+
+    def _set_geometry(self, K, C, ref_mic, what, wide):
+        """Checks C (and ref_mic, and D against `wide`) before any device work; sets channels (None for an int C),
+        C, M, D and the layout.  Errors: the stream's own for an int C, ragged._Layout's for a sequence."""
+        ragged = _is_ragged(C)
+        if ragged:
+            lay = _Layout(C, None, ref_mic)            # counts, K <= 16, D <= 16, ref_mic on every node
+            if lay.K != K:
+                raise ValueError("channels holds %d counts for K = %d nodes" % (lay.K, K))
+            self.channels, self.C = list(lay.channels), tuple(lay.channels)
+            D = max(lay.channels) + K - 1
+        else:
+            C = int(C)
+            D = C + K - 1
+            if D > 16:
+                raise NotImplementedError("the %s covers C + K - 1 <= 16 channels, got %d" % (what, D))
+        if D > 8 and not wide:
+            raise NotImplementedError("C + K - 1 = %d: the stream covers 9..16 channels with wide=True "
+                                      "(<= 8 without)" % D)
+        if not ragged:
+            _check_ref_mic(ref_mic, C)
+            lay = _Layout([C] * K, None, int(ref_mic))
+            self.channels, self.C = None, C
+        self.K, self.D, self.M, self._lay = K, D, sum(lay.channels), lay
+
+    def _make_groups(self, device):
+        self._groups = [_Group(C, nodes, self.K, self._lay, device) for C, nodes in self._lay.groups]
+
+    @property
+    def nodes(self):
+        """{C: the node indices of count C}, as online_tango_ragged returns them."""
+        return {g.C: list(g.nodes) for g in self._groups}
+
+    def _lead(self, first):
+        """The leading shape of an input: (first, K, C), or (first, M) packed."""
+        return (first, self.K, self.C) if self.channels is None else (first, self.M)
+
+    def _split(self, x):
+        """An input [B, K, C, ...] or packed [B, M, ...] (contiguous) -> per group [B, n_C, C, ...]."""
+        if self.channels is None:
+            return [x]
+        return [(x if g.n == self.K else x.index_select(1, g.rows)).view(x.shape[0], g.n, g.C, *x.shape[2:])
+                for g in self._groups]
+
+    def _join(self, parts):
+        """Per group [B, n_C, ...] -> [B, K, ...] over all nodes (one index_copy per group)."""
+        if len(parts) == 1:
+            return parts[0]
+        p0 = parts[0]
+        out = torch.empty((p0.shape[0], self.K) + tuple(p0.shape[2:]), dtype=p0.dtype, device=p0.device)
+        for g, p in zip(self._groups, parts):
+            out.index_copy_(1, g.idx, p)
+        return out
+
+    def _take(self, x, g):
+        """[B, K, ...] -> the nodes of group g, [B, n_C, ...]."""
+        return x if g.n == self.K else x.index_select(1, g.idx)
+
+    def _pack(self, parts):
+        """Per-group spectra [B, n_C, C, ...] -> mask_fn's Y: [B, K, C, ...], or packed [B, M, ...]."""
+        if self.channels is None:
+            return parts[0]
+        p0 = parts[0]
+        rest = tuple(p0.shape[3:])
+        if len(parts) == 1:
+            return p0.view((p0.shape[0], self.M) + rest)
+        out = torch.empty((p0.shape[0], self.M) + rest, dtype=p0.dtype, device=p0.device)
+        for g, p in zip(self._groups, parts):
+            out.index_copy_(1, g.rows, p.view((p.shape[0], g.n * g.C) + rest))
+        return out
+
+    def _plane(self, parts, mic):
+        """Microphone `mic` of every node, [B, K, ...], from per-group spectra [B, n_C, C, ...]."""
+        return self._join([_ref_plane(p, mic) for p in parts])
+
+    def _check_r0_kind(self, R0):
+        """R0's tensors (flat), checked for their kind: the pair (R_ss, R_nn) for an int C, a list of K pairs for a
+        sequence; ValueError / TypeError before any device work."""
+        if self.channels is None:
+            if not isinstance(R0, (tuple, list)) or len(R0) != 2:
+                raise ValueError("R0 must be the pair (R_ss, R_nn)")
+            flat = list(R0)
+        else:
+            if not isinstance(R0, (tuple, list)) or len(R0) != self.K or \
+                    any(not isinstance(p, (tuple, list)) or len(p) != 2 for p in R0):
+                raise ValueError("R0 must be a list of K = %d (R_ss, R_nn) pairs, one per node" % self.K)
+            flat = [r for p in R0 for r in p]
+        for r in flat:
+            if not isinstance(r, torch.Tensor) or not r.is_cuda:
+                raise TypeError("R0 must hold CUDA tensors (disco_b200 has no CPU path)")
+        return flat
+
+    def _check_r0_shapes(self, R0, first, device):
+        """R0's dtype, shapes and device: [first, K, F, C, C] per matrix, or [first, F, C_k, C_k] for node k."""
+        if self.channels is None:
+            R0, want = [R0], [(first, self.K, self.F, self.C, self.C)]
+        else:
+            want = [(first, self.F, c, c) for c in self.channels]
+        for k, (pair, w) in enumerate(zip(R0, want)):
+            for r in pair:
+                if r.dtype != torch.complex64 or tuple(r.shape) != w or r.device != device:
+                    raise ValueError("R0%s matrices must be complex64 [%s] on %s"
+                                     % ("" if self.channels is None else "[%d]" % k, ", ".join(map(str, w)), device))
+
+    def _r0_groups(self, R0):
+        """R0 -> per group the pair (R_ss, R_nn) [first, n_C, F, C, C] (fresh tensors)."""
+        if self.channels is None:
+            return [tuple(r.contiguous().clone() for r in R0)]
+        return [_group_R0(R0, g.nodes, self.K) for g in self._groups]
+
+
+class OnlineTangoStream(_Geometry):
     """B streams of K nodes x C microphones (D = C + K - 1 <= 8, or <= 16 with wide=True) that start together and
     advance in lockstep; two-step recursive Tango with the parameters and options of `online_tango`:
 
@@ -147,6 +303,15 @@ class OnlineTangoStream:
     z_y, zn [B, K, f, F] (step 1).  It returns frame-major float32 masks [B, K, f, F]; mask_w = None means mask_z.
     Precomputed masks are a slice by t0; a causal estimator reads Y, z_y and zn.  A call that completes no frame needs
     no mask_fn.
+
+    Ragged arrays: C may be a sequence of K per-node counts (channels, as in ragged.py; K <= 16, max(C_k) + K - 1 <=
+    16, ref_mic a microphone of every node).  Every chunk (and s_chunk, n_chunk) is then packed [B, M, n], M =
+    sum(channels), node k on rows off_k .. off_k + C_k - 1; mask_fn's Y is packed [B, M, f, F] (row r: packed
+    microphone r); R0 is a list of K pairs (R_ss, R_nn) [B, F, C_k, C_k], as online_tango_ragged takes it; W1 and W2
+    are dicts {C: [B, n_C, F, C]} and {C: [B, n_C, F, C + K - 1]} over the nodes of each count (`nodes`).  Every
+    other input and output keeps its shape, and the outputs equal online_tango_ragged on the whole signal.  wide=True
+    is needed as soon as one count's C_k + K - 1 exceeds 8.  Equal counts ([4, 4, 4, 4]) take packed chunks and
+    equal the int-C stream.
 
     filter_type, mu and rank reach both solves; mask_for_z is online_tango's exchange mode ('local', 'distant', and
     any other string but the ones below: 'previous', the unmasked z in both statistics).  With clean=True every push
@@ -172,77 +337,82 @@ class OnlineTangoStream:
 
     def __init__(self, B, K, C, n_fft=512, lambda_cor=0.95, block=8, lag=1, mu=1.0, rank=1, ref_mic=0, R0=None,
                  device=None, *, filter_type="gevd", mask_for_z="local", clean=False, vads=None, wide=False):
-        B, K, C = int(B), int(K), int(C)
-        if B < 1 or K < 1 or C < 1:
+        B, K = int(B), int(K)
+        if B < 1 or K < 1 or (not _is_ragged(C) and int(C) < 1):
             raise ValueError("B, K and C must be positive")
         _check_params(n_fft, block, lambda_cor, lag)
-        D = C + K - 1
-        if D > 16:
-            raise NotImplementedError("the stream covers C + K - 1 <= 16 channels, got %d" % D)
-        if D > 8 and not wide:
-            raise NotImplementedError("C + K - 1 = %d: the stream covers 9..16 channels with wide=True "
-                                      "(<= 8 without)" % D)
-        _check_ref_mic(ref_mic, C)
+        self._set_geometry(K, C, ref_mic, "stream", wide)
         clean = bool(clean) or vads is not None
         _check_options(filter_type, rank, mask_for_z, clean, vads)
-        if R0 is not None:
-            if not isinstance(R0, (tuple, list)) or len(R0) != 2:
-                raise ValueError("R0 must be the pair (R_ss, R_nn)")
-            for r in R0:
-                if not isinstance(r, torch.Tensor) or not r.is_cuda:
-                    raise TypeError("R0 must hold CUDA tensors (disco_b200 has no CPU path)")
-        device = _cuda_device(R0[0].device if device is None and R0 is not None else device, "stream")
+        flat = self._check_r0_kind(R0) if R0 is not None else None
+        device = _cuda_device(flat[0].device if device is None and R0 is not None else device, "stream")
         F, H, P = n_fft // 2 + 1, n_fft // 2, int(block)
+        self.B, self.F = B, F
         if R0 is not None:
-            for r in R0:
-                if r.dtype != torch.complex64 or tuple(r.shape) != (B, K, F, C, C) or r.device != device:
-                    raise ValueError("R0 matrices must be complex64 [%d, %d, %d, %d, %d] on %s" % (B, K, F, C, C, device))
-            R0 = tuple(r.contiguous().clone() for r in R0)
-        self.B, self.K, self.C, self.D, self.F = B, K, C, D, F
+            self._check_r0_shapes(R0, B, device)
         self.n_fft, self.block, self.lag = n_fft, P, int(lag)
         self.lambda_cor, self.mu, self.rank, self.ref_mic = float(lambda_cor), float(mu), rank, int(ref_mic)
         self.filter_type, self.mask_for_z, self.clean = filter_type, mask_for_z, clean
         self.vads = None if vads is None else tuple(vads)
         self.device = device
+        self._make_groups(device)
         f32, c64 = dict(dtype=torch.float32, device=device), dict(dtype=torch.complex64, device=device)
-        pair = lambda: [torch.zeros((B, K, C, n_fft), **f32), torch.zeros((B, K, C, n_fft), **f32)]   # in, out
-        self._hist = pair()
-        self._hist_sn = (pair(), pair()) if clean else None
-        self._none = torch.empty((B, K, C, 0), **f32)
+        self._oracle1 = "use_oracle_" in mask_for_z
+        R0s = self._r0_groups(R0) if R0 is not None else [None] * len(self._groups)
+        for g, r0 in zip(self._groups, R0s):
+            pair = lambda: [torch.zeros((B, g.n, g.C, n_fft), **f32), torch.zeros((B, g.n, g.C, n_fft), **f32)]
+            g.hist = pair()                                             # in, out
+            g.hist_sn = (pair(), pair()) if clean else None
+            # the open block's spectra, written in place run by run; the clean ones for the 'use_oracle_*' statistics
+            g.Yblk = torch.zeros((B, g.n, g.C, P, F), **c64)
+            g.SNblk = tuple(torch.zeros((B, g.n, g.C, P, F), **c64) for _ in range(2)) if self._oracle1 else None
+            # carried statistics: step 1 from R0; step 2 from R0 for a single node, from zeros otherwise
+            g.R1, g.R2 = r0, (r0 if K == 1 else None)
+            # solved filters by block index, kept while a later block still uses them; pass-through stand-ins
+            g.W1s, g.W2s = {}, {}
+            g.pass1 = torch.zeros((B, g.n, 1, F, g.C), **c64)
+            g.pass2 = torch.zeros((B, g.n, 1, F, g.D), **c64)
+        self._none = torch.empty(self._lead(B) + (0,), **f32)
         # one iSTFT carry per time signal: yf, or the six of TIME_NAMES
         self._carry = torch.zeros((len(TIME_NAMES), B, K, H) if clean else (B, K, H), **f32)
-        # the open block: its spectra, masks and (K > 1) step-1 outputs, written in place run by run; the clean
-        # spectra for the 'use_oracle_*' statistics, z_s and z_n for the exchange modes that read them
-        self._oracle1 = "use_oracle_" in mask_for_z
-        self._Yblk = torch.zeros((B, K, C, P, F), **c64)
+        # the open block over all K nodes: masks and (K > 1) step-1 outputs; z_s and z_n for the exchange modes that
+        # read them
         self._m1 = torch.zeros((B, K, P, F), **f32)
         self._m2 = torch.zeros((B, K, P, F), **f32)
         self._zblk = torch.zeros((B, K, P, F), **c64) if K > 1 else None
-        self._SNblk = tuple(torch.zeros((B, K, C, P, F), **c64) for _ in range(2)) if self._oracle1 else None
         self._zsnblk = None
         if K > 1 and mask_for_z in ("compressed", "use_oracle_zs"):
             self._zsnblk = tuple(torch.zeros((B, K, P, F), **c64) for _ in range(2))
-        # carried statistics: step 1 from R0; step 2 from R0 for a single node, from zeros otherwise
-        self._R1 = R0
-        self._R2 = R0 if K == 1 else None
-        # solved filters by block index, kept while a later block still uses them; pass-through stand-ins
-        self._W1s, self._W2s = {}, {}
-        self._pass1 = torch.zeros((B, K, 1, F, C), **c64)
-        self._pass2 = torch.zeros((B, K, 1, F, D), **c64)
         self._L = self._T = self._S = 0
         self._closed = False
 
     # ---------------------------------------------------------------- state
+    def _last_filters(self, step):
+        if not self._groups[0].W1s:
+            return None
+        Ws = {g.C: (g.W1s, g.W2s)[step][max(g.W1s)] for g in self._groups}
+        return Ws[self.C] if self.channels is None else Ws
+
     @property
     def W1(self):
         """Step-1 filters [B, K, F, C] of the last closed block (None before the first); block j's come into force for
-        block j + lag."""
-        return self._W1s[max(self._W1s)] if self._W1s else None
+        block j + lag.  With per-node counts: {C: [B, n_C, F, C]} over the nodes of each count."""
+        return self._last_filters(0)
 
     @property
     def W2(self):
-        """Step-2 filters [B, K, F, D] of the last closed block (None before the first)."""
-        return self._W2s[max(self._W2s)] if self._W2s else None
+        """Step-2 filters [B, K, F, D] of the last closed block (None before the first); with per-node counts
+        {C: [B, n_C, F, C + K - 1]}."""
+        return self._last_filters(1)
+
+    @property
+    def _R1(self):
+        """The carried step-1 statistics (R_ss, R_nn) of the first group (every node of an int-C stream)."""
+        return self._groups[0].R1
+
+    @property
+    def _R2(self):
+        return self._groups[0].R2
 
     @property
     def samples_in(self):
@@ -262,8 +432,8 @@ class OnlineTangoStream:
 
     # ---------------------------------------------------------------- public calls
     def push(self, y_chunk, mask_fn=None, *, s_chunk=None, n_chunk=None):
-        """Append y_chunk [B, K, C, n] float32 (n >= 0) to every stream, and s_chunk, n_chunk (its clean components,
-        shaped like it) to a stream with clean components; returns what became final (class doc)."""
+        """Append y_chunk [B, K, C, n] (packed: [B, M, n]) float32 (n >= 0) to every stream, and s_chunk, n_chunk (its
+        clean components, shaped like it) to a stream with clean components; returns what became final (class doc)."""
         self._check_open()
         self._check_chunk(y_chunk, "y_chunk")
         if self.clean:
@@ -304,8 +474,9 @@ class OnlineTangoStream:
             raise TypeError("%s must be a CUDA tensor (disco_b200 has no CPU path)" % name)
         if x.dtype != torch.float32:
             raise TypeError("%s must be float32, got %s" % (name, x.dtype))
-        if x.dim() != 4 or tuple(x.shape[:3]) != (self.B, self.K, self.C):
-            raise ValueError("%s shape %s, expected (%d, %d, %d, n)" % (name, tuple(x.shape), self.B, self.K, self.C))
+        lead = self._lead(self.B)
+        if x.dim() != len(lead) + 1 or tuple(x.shape[:-1]) != lead:
+            raise ValueError("%s shape %s, expected (%s, n)" % (name, tuple(x.shape), ", ".join(map(str, lead))))
         if x.device != self.device:
             raise ValueError("%s is on %s, the stream on %s" % (name, x.device, self.device))
 
@@ -324,7 +495,7 @@ class OnlineTangoStream:
             raise
 
     def _in_force(self, Ws, stand_in, j):
-        """(W [B, K, 1, F, D], lag argument of filter_sum_blocks) for the frames of block j: the filter of block
+        """(W [B, n, 1, F, D], lag argument of filter_sum_blocks) for the frames of block j: the filter of block
         j - lag, or, while that does not exist, the kernel's own pass-through of the reference channel."""
         jw = j - self.lag
         return (stand_in, 1) if jw < 0 else (Ws[jw].unsqueeze(2), 0)
@@ -333,73 +504,89 @@ class OnlineTangoStream:
         """Statistics and filters of block j once the masks of its nb frames are in (nb < block: the final, partial
         block, whose recursion step is lambda^nb, as in the whole-signal scan).  The statistics are online_tango's
         for the stream's mask_for_z: the masked scans for 'local', the split scans of [mask Y ; z_rs] and
-        [(1 - mask) Y ; z_rn] otherwise, and those of S and N for step 1 under 'use_oracle_*'."""
-        P, lam, n_fft, K = self.block, self.lambda_cor, self.n_fft, self.K
+        [(1 - mask) Y ; z_rn] otherwise, and those of S and N for step 1 under 'use_oracle_*'.  Each stage runs once
+        per group, step 2 reading the z of all K nodes."""
+        P, lam, n_fft, K, groups = self.block, self.lambda_cor, self.n_fft, self.K, self._groups
         cut = (lambda b: b) if nb == P else (lambda b: None if b is None else b[..., :nb, :].contiguous())
-        Yb, m1, m2, zb = cut(self._Yblk), cut(self._m1), cut(self._m2), cut(self._zblk)
-        Sb, Nb = (cut(b) for b in self._SNblk) if self._SNblk is not None else (None, None)
+        m1, m2, zb = cut(self._m1), cut(self._m2), cut(self._zblk)
+        blk = [(cut(g.Yblk),) + (tuple(cut(b) for b in g.SNblk) if g.SNblk is not None else (None, None))
+               for g in groups]
         zsb, znb = (cut(b) for b in self._zsnblk) if self._zsnblk is not None else (None, None)
         # scm_recursive writes fresh matrices, so its output never aliases the carried R0 it reads
-        if self._oracle1:
-            Rs1, Rn1 = _split_scans(Sb, Nb, None, None, None, lam, P, self._R1, n_fft)
-        else:
-            Rs1, Rn1 = ops.scm_recursive(Yb, m1, None, lam, P, 2, self._R1, n_fft)
-        if self.mask_for_z == "local":
-            Rs2, Rn2 = ops.scm_recursive(Yb, m2, zb, lam, P, 2, self._R2, n_fft)
-        else:
-            # what the other nodes contribute; a single node has none (online_tango reads its own channels only)
-            z_rs = z_rn = None
-            if K > 1:
-                kind = self.vads[0] if self.vads is not None else "irm1"
-                z_rs, z_rn = _z_for_stats(self.mask_for_z, (kind, kind), zb, m2, zsb, znb,
-                                          lambda: (_ref_plane(Sb, self.ref_mic), _ref_plane(Nb, self.ref_mic)))
-            Rs2, Rn2 = _split_scans(Yb, Yb, z_rs, z_rn, m2, lam, P, self._R2, n_fft)
-        self._R1, self._R2 = (Rs1[:, :, 0], Rn1[:, :, 0]), (Rs2[:, :, 0], Rn2[:, :, 0])
-        self._W1s[j] = ops.mwf_solve(Rs1, Rn1, self.mu, self.filter_type, self.rank)[0][:, :, 0]
-        self._W2s[j] = ops.mwf_solve(Rs2, Rn2, self.mu, self.filter_type, self.rank)[0][:, :, 0]
-        for Ws in (self._W1s, self._W2s):
-            for old in [i for i in Ws if i < j + 1 - self.lag]:
-                del Ws[old]
+        st1 = []
+        for g, (Yb, Sb, Nb) in zip(groups, blk):
+            if self._oracle1:
+                st1.append(_split_scans(Sb, Nb, None, None, None, lam, P, g.R1, n_fft))
+            else:
+                st1.append(ops.scm_recursive(Yb, self._take(m1, g), None, lam, P, 2, g.R1, n_fft))
+        # what the other nodes contribute; a single node has none (online_tango reads its own channels only)
+        z_rs = z_rn = None
+        if self.mask_for_z != "local" and K > 1:
+            kind = self.vads[0] if self.vads is not None else "irm1"
+            z_rs, z_rn = _z_for_stats(self.mask_for_z, (kind, kind), zb, m2, zsb, znb,
+                                      lambda: (self._plane([b[1] for b in blk], self.ref_mic),
+                                               self._plane([b[2] for b in blk], self.ref_mic)))
+        st2 = []
+        for g, (Yb, _, _) in zip(groups, blk):
+            if self.mask_for_z == "local":
+                st2.append(ops.scm_recursive(Yb, self._take(m2, g), zb, lam, P, 2, g.R2, n_fft, node_sel=g.sel))
+            else:
+                st2.append(_split_scans(Yb, Yb, z_rs, z_rn, self._take(m2, g), lam, P, g.R2, n_fft, node_sel=g.sel))
+        for g, (Rs1, Rn1), (Rs2, Rn2) in zip(groups, st1, st2):
+            g.R1, g.R2 = (Rs1[:, :, 0], Rn1[:, :, 0]), (Rs2[:, :, 0], Rn2[:, :, 0])
+            g.W1s[j] = ops.mwf_solve(Rs1, Rn1, self.mu, self.filter_type, self.rank)[0][:, :, 0]
+            g.W2s[j] = ops.mwf_solve(Rs2, Rn2, self.mu, self.filter_type, self.rank)[0][:, :, 0]
+            for Ws in (g.W1s, g.W2s):
+                for old in [i for i in Ws if i < j + 1 - self.lag]:
+                    del Ws[old]
 
     def _advance(self, chunk, sn, L1, T1, S1, mask_fn, final):
-        B, K, F, P, n_fft, ref = self.B, self.K, self.F, self.block, self.n_fft, self.ref_mic
+        B, K, F, P, n_fft, ref, groups = self.B, self.K, self.F, self.block, self.n_fft, self.ref_mic, self._groups
         T0, S0 = self._T, self._S
-        hist_in, hist_out = self._hist
         clean = sn is not None
         update = chunk.shape[-1] > 0          # the history moves with every sample that arrives
+        xs = self._split(chunk)
+        xsn = list(zip(*(self._split(x) for x in sn))) if clean else [None] * len(groups)   # per group: (s, n)
         x_time = torch.empty(((len(TIME_NAMES),) if clean else ()) + (B, K, S1 - S0), dtype=torch.float32,
                              device=self.device)
         names = ["z_y", "zn", "yf"] + (["z_s", "z_n", "sf", "nf"] if clean else []) + \
             (["masks_z", "mask_w"] if self.vads is not None else [])
         parts = []
         if T1 == T0 and update:
-            ops.stream_stft(hist_in, chunk, L1, T0, 0, n_fft, hist_out=hist_out)
-            if clean:
-                for x, (h_in, h_out) in zip(sn, self._hist_sn):
-                    ops.stream_stft(h_in, x, L1, T0, 0, n_fft, hist_out=h_out)
+            for g, x, xc in zip(groups, xs, xsn):
+                ops.stream_stft(g.hist[0], x, L1, T0, 0, n_fft, hist_out=g.hist[1])
+                if clean:
+                    for x2, (h_in, h_out) in zip(xc, g.hist_sn):
+                        ops.stream_stft(h_in, x2, L1, T0, 0, n_fft, hist_out=h_out)
         t = T0
         while t < T1:
             j, slot = divmod(t, P)
             f = min(T1, (j + 1) * P) - t
             last = t + f == T1
-            Y = ops.stream_stft(hist_in, chunk, L1, t, f, n_fft, hist_out=hist_out if (last and update) else None,
-                                Y_blk=self._Yblk, blk_slot=slot, final=final)
-            if clean:
-                # S, N: one transform each, as online_tango takes them (the pairing of signals decides the bits)
-                S, N = (ops.stream_stft(h_in, x, L1, t, f, n_fft, hist_out=h_out if (last and update) else None,
-                                        Y_blk=None if self._SNblk is None else self._SNblk[i], blk_slot=slot,
-                                        final=final)
-                        for i, (x, (h_in, h_out)) in enumerate(zip(sn, self._hist_sn)))
-            W1, lg1 = self._in_force(self._W1s, self._pass1, j)
-            z, zn = ops.filter_sum_blocks(W1, Y, None, P, lg1, True, ref, n_fft)
-            W2, lg2 = self._in_force(self._W2s, self._pass2, j)
-            yf, _ = ops.filter_sum_blocks(W2, Y, z if K > 1 else None, P, lg2, True, ref, n_fft)
+            keep = last and update
+            Ys, SNs = [], []
+            for g, x, xc in zip(groups, xs, xsn):
+                Ys.append(ops.stream_stft(g.hist[0], x, L1, t, f, n_fft, hist_out=g.hist[1] if keep else None,
+                                          Y_blk=g.Yblk, blk_slot=slot, final=final))
+                if clean:
+                    # S, N: one transform each, as online_tango takes them (the pairing of signals decides the bits)
+                    SNs.append(tuple(ops.stream_stft(h_in, x2, L1, t, f, n_fft, hist_out=h_out if keep else None,
+                                                     Y_blk=None if g.SNblk is None else g.SNblk[i], blk_slot=slot,
+                                                     final=final)
+                                     for i, (x2, (h_in, h_out)) in enumerate(zip(xc, g.hist_sn))))
+            Ws = [(self._in_force(g.W1s, g.pass1, j), self._in_force(g.W2s, g.pass2, j)) for g in groups]
+            st1 = [ops.filter_sum_blocks(W1, Y, None, P, lg1, True, ref, n_fft) for ((W1, lg1), _), Y in zip(Ws, Ys)]
+            z, zn = self._join([a[0] for a in st1]), self._join([a[1] for a in st1])
+            yf = self._join([ops.filter_sum_blocks(W2, Y, z if K > 1 else None, P, lg2, True, ref, n_fft,
+                                                   node_sel=g.sel)[0]
+                             for g, (_, (W2, lg2)), Y in zip(groups, Ws, Ys)])
             if self.vads is None:
-                mz, mw = _check_masks(mask_fn(t, Y, z, zn), (B, K, f, F), self.device)
+                mz, mw = _check_masks(mask_fn(t, self._pack(Ys), z, zn), (B, K, f, F), self.device)
             else:
-                # tf_mask is elementwise, so the run's masks are those of the whole signal; S stands in for the time
-                # signal, which only 'ivad' reads
-                mz, mw = _clean_masks(S, N, S, self.vads, ref, n_fft)
+                # tf_mask is elementwise, so the run's masks are those of the whole signal (tango._clean_masks)
+                spectra = lambda c: (self._plane([a[0] for a in SNs], c), self._plane([a[1] for a in SNs], c))
+                mz = _step1_mask(self.vads[0], None, lambda: spectra(ref), None, None, n_fft)
+                mw = _step2_mask(self.vads, None, mz, lambda: spectra(0), None, n_fft, ref_mic=ref)
             self._m1[:, :, slot:slot + f].copy_(mz)
             self._m2[:, :, slot:slot + f].copy_(mw)
             if K > 1:
@@ -407,10 +594,13 @@ class OnlineTangoStream:
             part = [z, zn, yf]
             if clean:
                 # the diagnostics of online_tango: W1 on S, N; W2 on [S_own ; z_s], [N_own ; z_n]
-                z_s = ops.filter_sum_blocks(W1, S, None, P, lg1, True, ref, n_fft)[0]
-                z_n = ops.filter_sum_blocks(W1, N, None, P, lg1, True, ref, n_fft)[0]
-                sf = ops.filter_sum_blocks(W2, S, z_s if K > 1 else None, P, lg2, True, ref, n_fft)[0]
-                nf = ops.filter_sum_blocks(W2, N, z_n if K > 1 else None, P, lg2, True, ref, n_fft)[0]
+                zsn = [tuple(ops.filter_sum_blocks(W1, X, None, P, lg1, True, ref, n_fft)[0] for X in sng)
+                       for ((W1, lg1), _), sng in zip(Ws, SNs)]
+                z_s, z_n = self._join([a[0] for a in zsn]), self._join([a[1] for a in zsn])
+                sfn = [tuple(ops.filter_sum_blocks(W2, X, Zx if K > 1 else None, P, lg2, True, ref, n_fft,
+                                                   node_sel=g.sel)[0] for X, Zx in zip(sng, (z_s, z_n)))
+                       for g, (_, (W2, lg2)), sng in zip(groups, Ws, SNs)]
+                sf, nf = self._join([a[0] for a in sfn]), self._join([a[1] for a in sfn])
                 if self._zsnblk is not None:
                     self._zsnblk[0][:, :, slot:slot + f].copy_(z_s)
                     self._zsnblk[1][:, :, slot:slot + f].copy_(z_n)
@@ -428,10 +618,11 @@ class OnlineTangoStream:
             parts.append(part)
             t += f
         if update:
-            self._hist.reverse()
-            if clean:
-                for h in self._hist_sn:
-                    h.reverse()
+            for g in groups:
+                g.hist.reverse()
+                if clean:
+                    for h in g.hist_sn:
+                        h.reverse()
         self._L, self._T, self._S = L1, T1, S1
         out = {"t0": T0}
         for i, nm in enumerate(names):
@@ -467,7 +658,7 @@ def pool_rounds(T0, T1, block):
     return np.minimum(start, T1), n
 
 
-class OnlineTangoPool:
+class OnlineTangoPool(_Geometry):
     """S slots, each an independent online Tango stream of K nodes x C microphones that opens, advances and closes on
     its own; the parameters are those of OnlineTangoStream, filter_type and the exchange modes that need no clean
     components ('local', 'distant', 'previous') included, and one pool has one geometry (D = C + K - 1 <= 16):
@@ -483,6 +674,11 @@ class OnlineTangoPool:
     signal and ops.istft of its yf), with the masks mask_fn returned -- whatever the other slots do, the slot's index,
     and the cut of its samples into pushes.  A slot's K C signals are paired into transforms inside the slot, as the single stream pairs them.
 
+    Ragged arrays: C may be a sequence of K per-node counts, as for OnlineTangoStream.  y is then packed [S, M, n_max];
+    mask_fn's Y is packed [S, M, f_max, F]; open takes R0 as a list of K pairs [len(slots), F, C_k, C_k]; filters
+    returns the dicts ({C: [n_C, F, C]}, {C: [n_C, F, C + K - 1]}) over the nodes of each count (`nodes`).  A slot's
+    signals pair inside each of its groups, so it equals OnlineTangoStream(1, K, channels).
+
     mask_fn(t0, n_fr, Y, z_y, zn) -> (mask_z, mask_w) is called once per round: every slot's frames of the call are
     cut into runs that never cross its block boundary (pool_rounds), and round r holds every slot's r-th run.  t0 and
     n_fr are host int arrays [S] (n_fr[s] = 0: no frames of slot s in the round); Y is [S, K, C, f_max, F], z_y and zn
@@ -497,23 +693,21 @@ class OnlineTangoPool:
 
     def __init__(self, S, K, C, n_fft=512, lambda_cor=0.95, block=8, lag=1, mu=1.0, rank=1, ref_mic=0, device=None,
                  *, filter_type="gevd", mask_for_z="local"):
-        S, K, C = int(S), int(K), int(C)
-        if S < 1 or K < 1 or C < 1:
+        S, K = int(S), int(K)
+        if S < 1 or K < 1 or (not _is_ragged(C) and int(C) < 1):
             raise ValueError("S, K and C must be positive")
         _check_params(n_fft, block, lambda_cor, lag)
-        D = C + K - 1
-        if D > 16:
-            raise NotImplementedError("the pool covers C + K - 1 <= 16 channels, got %d" % D)
-        _check_ref_mic(ref_mic, C)
+        self._set_geometry(K, C, ref_mic, "pool", True)
         _check_options(filter_type, rank, mask_for_z, False, None)
         if S > 65535:
             raise ValueError("at most 65535 slots")
         device = _cuda_device(device, "pool")
-        self.S, self.K, self.C, self.D, self.F = S, K, C, D, n_fft // 2 + 1
+        self.S, self.F = S, n_fft // 2 + 1
         self.n_fft, self.block, self.lag = n_fft, int(block), int(lag)
         self.lambda_cor, self.mu, self.rank, self.ref_mic = float(lambda_cor), float(mu), rank, int(ref_mic)
         self.filter_type, self.mask_for_z = filter_type, mask_for_z
         self.device = device
+        self._make_groups(device)
         # host state per slot
         self._open = np.zeros(S, dtype=bool)
         self._L = np.zeros(S, dtype=np.int64)          # samples in
@@ -527,28 +721,30 @@ class OnlineTangoPool:
         """Device state, allocated on the first open."""
         if self._bufs:
             return
-        S, K, C, D, F, P, N, dev = self.S, self.K, self.C, self.D, self.F, self.block, self.n_fft, self.device
+        S, K, F, P, N, dev = self.S, self.K, self.F, self.block, self.n_fft, self.device
         f32, c64 = dict(dtype=torch.float32, device=dev), dict(dtype=torch.complex64, device=dev)
-        self._hist = torch.zeros((2, S, K, C, N), **f32)
         self._carry = torch.zeros((S, K, N // 2), **f32)
-        # the open block of every slot: its spectra, masks and (K > 1) step-1 outputs
-        self._Yblk = torch.zeros((S, K, C, P, F), **c64)
+        # the open block of every slot over all K nodes: masks and (K > 1) step-1 outputs
         self._m1 = torch.zeros((S, K, P, F), **f32)
         self._m2 = torch.zeros((S, K, P, F), **f32)
         self._zblk = torch.zeros((S, K, P, F), **c64) if K > 1 else None
-        # carried statistics (zeros stand for "none yet": the scan's R_(-1) is 0 either way)
-        self._R1 = (torch.zeros((S, K, F, C, C), **c64), torch.zeros((S, K, F, C, C), **c64))
-        self._R2 = (torch.zeros((S, K, F, D, D), **c64), torch.zeros((S, K, F, D, D), **c64))
-        # ring of the last lag + 1 filters: block j's at j % (lag + 1).  Entries of blocks before the first hold the
-        # pass-through of the reference channel, stored as (e_ref, -0) so that the kernel's conjugate is exactly the
-        # weight vector of filter_sum_blocks' own pass-through.
-        self._W1 = torch.zeros((S, self.lag + 1, K, F, C), **c64)
-        self._W2 = torch.zeros((S, self.lag + 1, K, F, D), **c64)
-        self._pass = []
-        for d in (C, D):
-            re = torch.zeros((K, F, d), **f32)
-            re[..., self.ref_mic] = 1.0
-            self._pass.append(torch.complex(re, torch.full_like(re, -0.0)))
+        for g in self._groups:
+            C, D, n = g.C, g.D, g.n
+            g.hist = torch.zeros((2, S, n, C, N), **f32)
+            g.Yblk = torch.zeros((S, n, C, P, F), **c64)      # the open block's spectra
+            # carried statistics (zeros stand for "none yet": the scan's R_(-1) is 0 either way)
+            g.R1 = (torch.zeros((S, n, F, C, C), **c64), torch.zeros((S, n, F, C, C), **c64))
+            g.R2 = (torch.zeros((S, n, F, D, D), **c64), torch.zeros((S, n, F, D, D), **c64))
+            # ring of the last lag + 1 filters: block j's at j % (lag + 1).  Entries of blocks before the first hold
+            # the pass-through of the reference channel, stored as (e_ref, -0) so that the kernel's conjugate is
+            # exactly the weight vector of filter_sum_blocks' own pass-through.
+            g.W1 = torch.zeros((S, self.lag + 1, n, F, C), **c64)
+            g.W2 = torch.zeros((S, self.lag + 1, n, F, D), **c64)
+            g.pass_ = []
+            for d in (C, D):
+                re = torch.zeros((n, F, d), **f32)
+                re[..., self.ref_mic] = 1.0
+                g.pass_.append(torch.complex(re, torch.full_like(re, -0.0)))
         self._bufs = True
 
     # ---------------------------------------------------------------- state
@@ -569,55 +765,58 @@ class OnlineTangoPool:
 
     def filters(self, slot):
         """(W1 [K, F, C], W2 [K, F, D]) of the slot's last closed block (in force from block j + lag), or None before
-        its first; kept after close until the slot is opened again."""
+        its first; kept after close until the slot is opened again.  With per-node counts: ({C: [n_C, F, C]},
+        {C: [n_C, F, C + K - 1]})."""
         s = int(self._slot_list([slot])[0])
         if self._nclosed[s] == 0:
             return None
         pos = int((self._nclosed[s] - 1) % (self.lag + 1))
-        return self._W1[s, pos].clone(), self._W2[s, pos].clone()
+        Ws = {g.C: (g.W1[s, pos].clone(), g.W2[s, pos].clone()) for g in self._groups}
+        if self.channels is None:
+            return Ws[self.C]
+        return {C: w[0] for C, w in Ws.items()}, {C: w[1] for C, w in Ws.items()}
 
     # ---------------------------------------------------------------- public calls
     def open(self, slots, R0=None):
         """Open free slots: every slot starts a new stream (history, block buffers, filters and iSTFT carry reset; the
-        carried matrices from R0, or zeros).  R0 = (R_ss, R_nn), complex64 [len(slots), K, F, C, C]."""
+        carried matrices from R0, or zeros).  R0 = (R_ss, R_nn), complex64 [len(slots), K, F, C, C] (per-node counts:
+        a list of K pairs [len(slots), F, C_k, C_k])."""
         idx = self._slot_list(slots)
         if self._open[idx].any():
             raise ValueError("slot %d is already open" % int(idx[self._open[idx]][0]))
-        K, C, F = self.K, self.C, self.F
         if R0 is not None:
-            if not isinstance(R0, (tuple, list)) or len(R0) != 2:
-                raise ValueError("R0 must be the pair (R_ss, R_nn)")
-            for r in R0:
-                if not isinstance(r, torch.Tensor) or not r.is_cuda:
-                    raise TypeError("R0 must hold CUDA tensors (disco_b200 has no CPU path)")
-                if r.dtype != torch.complex64 or tuple(r.shape) != (len(idx), K, F, C, C) or r.device != self.device:
-                    raise ValueError("R0 matrices must be complex64 [%d, %d, %d, %d, %d] on %s"
-                                     % (len(idx), K, F, C, C, self.device))
+            self._check_r0_kind(R0)
+            self._check_r0_shapes(R0, len(idx), self.device)
         if len(idx) == 0:
             return
         self._alloc()
+        K = self.K
         i = torch.from_numpy(idx).to(self.device)
-        self._hist[:, i] = 0
         self._carry[i] = 0
-        for buf in (self._Yblk, self._m1, self._m2, self._zblk):
+        for buf in (self._m1, self._m2, self._zblk):
             if buf is not None:
                 buf[i] = 0
-        for w in range(2):
-            self._R1[w][i] = 0 if R0 is None else R0[w]
-            self._R2[w][i] = R0[w] if (R0 is not None and K == 1) else 0   # step 2 of a single node starts from R0
-        self._W1[i] = self._pass[0]
-        self._W2[i] = self._pass[1]
+        R0s = self._r0_groups(R0) if R0 is not None else [None] * len(self._groups)
+        for g, r0 in zip(self._groups, R0s):
+            g.hist[:, i] = 0
+            g.Yblk[i] = 0
+            for w in range(2):
+                g.R1[w][i] = 0 if r0 is None else r0[w]
+                g.R2[w][i] = r0[w] if (r0 is not None and K == 1) else 0   # step 2 of a single node starts from R0
+            g.W1[i] = g.pass_[0]
+            g.W2[i] = g.pass_[1]
         self._open[idx] = True
         for a in (self._L, self._T, self._S, self._par, self._nclosed):
             a[idx] = 0
 
     def push(self, y, n, mask_fn):
-        """Append y[s, :, :, :n[s]] to slot s (y [S, K, C, n_max] float32 CUDA; n host ints, 0 <= n[s] <= n_max, and
-        0 for free slots); returns what became final (class doc)."""
+        """Append y[s, ..., :n[s]] to slot s (y [S, K, C, n_max], packed [S, M, n_max], float32 CUDA; n host ints,
+        0 <= n[s] <= n_max, and 0 for free slots); returns what became final (class doc)."""
         if not isinstance(y, torch.Tensor):
             raise TypeError("y must be a CUDA tensor (disco_b200 has no CPU path)")
-        if y.dim() != 4 or tuple(y.shape[:3]) != (self.S, self.K, self.C):
-            raise ValueError("y shape %s, expected (%d, %d, %d, n_max)" % (tuple(y.shape), self.S, self.K, self.C))
+        lead = self._lead(self.S)
+        if y.dim() != len(lead) + 1 or tuple(y.shape[:-1]) != lead:
+            raise ValueError("y shape %s, expected (%s, n_max)" % (tuple(y.shape), ", ".join(map(str, lead))))
         n_max = y.shape[-1]
         n = np.asarray(n)
         if n.dtype.kind not in "iu" or n.shape != (self.S,):
@@ -653,7 +852,7 @@ class OnlineTangoPool:
         T1, S1 = self._T.copy(), self._S.copy()
         T1[idx] = 1 + self._L[idx] // H
         S1[idx] = self._L[idx]
-        chunk = torch.empty((self.S, self.K, self.C, 0), dtype=torch.float32, device=self.device)
+        chunk = torch.empty(self._lead(self.S) + (0,), dtype=torch.float32, device=self.device)
         out = self._run(chunk, np.zeros(self.S, dtype=np.int64), self._L.copy(), T1, S1, final, mask_fn)
         self._open[idx] = False
         return out
@@ -680,31 +879,43 @@ class OnlineTangoPool:
 
     def _close_blocks(self, cl, nb, ci):
         """Statistics and filters of the open block of the slots `cl` (ci: the same indices on the device) once the
-        masks of its nb[s] frames are in (nb < block: the final, partial block, whose recursion step is lambda^nb)."""
-        P, lam, n_fft = self.block, self.lambda_cor, self.n_fft
-        Yb, m1, m2 = self._Yblk[ci], self._m1[ci], self._m2[ci]
+        masks of its nb[s] frames are in (nb < block: the final, partial block, whose recursion step is lambda^nb).
+        Each stage runs once per group, step 2 reading the z of all K nodes."""
+        P, lam, n_fft, groups = self.block, self.lambda_cor, self.n_fft, self._groups
+        m1, m2 = self._m1[ci], self._m2[ci]
         zb = self._zblk[ci] if self.K > 1 else None
-        R1 = (self._R1[0][ci], self._R1[1][ci])
-        R2 = (self._R2[0][ci], self._R2[1][ci])
-        Rs1, Rn1 = ops.scm_recursive(Yb, m1, None, lam, P, 2, R1, n_fft, frames=nb)
-        if self.mask_for_z == "local":
-            Rs2, Rn2 = ops.scm_recursive(Yb, m2, zb, lam, P, 2, R2, n_fft, frames=nb)
-        else:
-            z_rs, z_rn = (None, None) if zb is None else _z_for_stats(self.mask_for_z, None, zb, m2, None, None, None)
-            Rs2, Rn2 = _split_scans(Yb, Yb, z_rs, z_rn, m2, lam, P, R2, n_fft, frames=nb)
-        W1 = ops.mwf_solve(Rs1, Rn1, self.mu, self.filter_type, self.rank)[0][:, :, 0]
-        W2 = ops.mwf_solve(Rs2, Rn2, self.mu, self.filter_type, self.rank)[0][:, :, 0]
-        for R, new in ((self._R1, (Rs1, Rn1)), (self._R2, (Rs2, Rn2))):
-            R[0][ci] = new[0][:, :, 0]
-            R[1][ci] = new[1][:, :, 0]
-        pos = torch.from_numpy(self._nclosed[cl] % (self.lag + 1)).to(self.device)
-        self._W1[ci, pos] = W1
-        self._W2[ci, pos] = W2
+        Ybs = [g.Yblk[ci] for g in groups]
+        st1 = [ops.scm_recursive(Yb, self._take(m1, g), None, lam, P, 2, (g.R1[0][ci], g.R1[1][ci]), n_fft,
+                                 frames=nb) for g, Yb in zip(groups, Ybs)]
+        z_rs = z_rn = None
+        if self.mask_for_z != "local" and zb is not None:
+            z_rs, z_rn = _z_for_stats(self.mask_for_z, None, zb, m2, None, None, None)
+        st2 = []
+        for g, Yb in zip(groups, Ybs):
+            R2 = (g.R2[0][ci], g.R2[1][ci])
+            if self.mask_for_z == "local":
+                st2.append(ops.scm_recursive(Yb, self._take(m2, g), zb, lam, P, 2, R2, n_fft, node_sel=g.sel,
+                                             frames=nb))
+            else:
+                st2.append(_split_scans(Yb, Yb, z_rs, z_rn, self._take(m2, g), lam, P, R2, n_fft, frames=nb,
+                                        node_sel=g.sel))
+        pos = None
+        for g, (Rs1, Rn1), (Rs2, Rn2) in zip(groups, st1, st2):
+            W1 = ops.mwf_solve(Rs1, Rn1, self.mu, self.filter_type, self.rank)[0][:, :, 0]
+            W2 = ops.mwf_solve(Rs2, Rn2, self.mu, self.filter_type, self.rank)[0][:, :, 0]
+            for R, new in ((g.R1, (Rs1, Rn1)), (g.R2, (Rs2, Rn2))):
+                R[0][ci] = new[0][:, :, 0]
+                R[1][ci] = new[1][:, :, 0]
+            if pos is None:
+                pos = torch.from_numpy(self._nclosed[cl] % (self.lag + 1)).to(self.device)
+            g.W1[ci, pos] = W1
+            g.W2[ci, pos] = W2
         self._nclosed[cl] += 1
 
     def _advance(self, chunk, n, L1, T1, S1, final, mask_fn):
         S, K, F, P, lag, n_fft, ref, dev = (self.S, self.K, self.F, self.block, self.lag, self.n_fft, self.ref_mic,
                                             self.device)
+        groups = self._groups
         T0, S0 = self._T.copy(), self._S.copy()
         frames, samples = T1 - T0, S1 - S0
         starts, runs = pool_rounds(T0, T1, P)
@@ -713,20 +924,22 @@ class OnlineTangoPool:
         out = [torch.zeros((S, K, f_call, F), **c64) for _ in range(3)]        # z_y, zn, yf
         yf_time = torch.zeros((S, K, int(samples.max())), dtype=torch.float32, device=dev)
         write = n > 0
+        xs = self._split(chunk)
         stft_rec = np.zeros((S, len(ops.STFT_SLOT_FIELDS)), dtype=np.int64)
         stft_rec[:, 0], stft_rec[:, 1], stft_rec[:, 5], stft_rec[:, 6] = L1, n, final, self._par
         istft_rec = np.zeros((S, len(ops.ISTFT_SLOT_FIELDS)), dtype=np.int64)
         istft_rec[:, 2], istft_rec[:, 4] = L1, S0
         if len(runs) == 0 and write.any():       # no frame completes: only the history moves
             stft_rec[:, 2], stft_rec[:, 7] = T0, write
-            ops.stream_stft_slots(self._hist, chunk, stft_rec, 0, n_fft)
+            for g, x in zip(groups, xs):
+                ops.stream_stft_slots(g.hist, x, stft_rec, 0, n_fft)
         for r in range(len(runs)):
             t0, nr = starts[r], runs[r]
             act = np.nonzero(nr)[0]
             fr, f = nr[act], int(nr.max())
             blk = np.where(nr > 0, t0 % P, 0)
             stft_rec[:, 2], stft_rec[:, 3], stft_rec[:, 4], stft_rec[:, 7] = t0, nr, blk, write if r == 0 else 0
-            Y = ops.stream_stft_slots(self._hist, chunk, stft_rec, f, n_fft, Y_blk=self._Yblk)
+            Ys = [ops.stream_stft_slots(g.hist, x, stft_rec, f, n_fft, Y_blk=g.Yblk) for g, x in zip(groups, xs)]
             # one host -> device copy per round: active slots, ring positions, and the (slot, frame) pairs of the run
             s_idx = np.repeat(act, fr)
             a_idx = np.repeat(np.arange(len(act)), fr)
@@ -738,17 +951,20 @@ class OnlineTangoPool:
             ai, pi = d[:na], d[na:2 * na]
             si, aj, ii, bi, oi = (d[2 * na + k * nf:2 * na + (k + 1) * nf] for k in range(5))
             every = na == S
-            Ya = Y if every else Y[ai]
+            Yas = Ys if every else [Y[ai] for Y in Ys]
             # step 1 and step 2 with the filter in force, W_(j - lag) (the pass-through stand-in before the first)
-            z, zn = ops.filter_sum_blocks(self._W1[ai, pi].unsqueeze(2), Ya, None, P, 0, True, ref, n_fft, frames=fr)
-            yf, _ = ops.filter_sum_blocks(self._W2[ai, pi].unsqueeze(2), Ya, z if K > 1 else None, P, 0, True, ref,
-                                          n_fft, frames=fr)
+            st1 = [ops.filter_sum_blocks(g.W1[ai, pi].unsqueeze(2), Ya, None, P, 0, True, ref, n_fft, frames=fr)
+                   for g, Ya in zip(groups, Yas)]
+            z, zn = self._join([a[0] for a in st1]), self._join([a[1] for a in st1])
+            yf = self._join([ops.filter_sum_blocks(g.W2[ai, pi].unsqueeze(2), Ya, z if K > 1 else None, P, 0, True,
+                                                   ref, n_fft, node_sel=g.sel, frames=fr)[0]
+                             for g, Ya in zip(groups, Yas)])
             if every:
                 zf, znf, yff = z, zn, yf
             else:
                 zf, znf, yff = (torch.zeros((S, K, f, F), **c64) for _ in range(3))
                 zf[ai], znf[ai], yff[ai] = z, zn, yf
-            mz, mw = _check_masks(mask_fn(t0.copy(), nr.copy(), Y, zf, znf), (S, K, f, F), dev)
+            mz, mw = _check_masks(mask_fn(t0.copy(), nr.copy(), self._pack(Ys), zf, znf), (S, K, f, F), dev)
             self._m1[si, :, bi] = mz[si, :, ii]
             self._m2[si, :, bi] = mw[si, :, ii]
             if K > 1:
