@@ -31,7 +31,7 @@ buffers that span all K nodes (masks, z, outputs) are assembled with index_copy.
 import numpy as np
 import torch
 
-from . import ops
+from . import ops, stream_state
 from .ragged import _Layout, _group_R0
 from .tango import _ORACLE_SIGS, _mask_kind, _ref_plane, _step1_mask, _step2_mask, _z_for_stats
 
@@ -297,6 +297,8 @@ class OnlineTangoStream(_Geometry):
         s = OnlineTangoStream(B, K, C, n_fft=512, lambda_cor=0.95, block=8, lag=1)
         out = s.push(y_chunk, mask_fn)     # y_chunk [B, K, C, n] float32 CUDA, any n >= 0
         out = s.flush(mask_fn)             # end of the stream: the last frame and the remaining samples
+        st = s.state()                     # or, at any point: save the session (stream_state) ...
+        s2 = OnlineTangoStream.from_state(st)   # ... and resume it, here or elsewhere, bit for bit
 
     mask_fn(t0, Y, z_y, zn) -> (mask_z, mask_w) is called once for each run of newly completed frames [t0, t0 + f),
     after the run's step-1 outputs exist and before any later frame is filtered, with Y [B, K, C, f, F] (the STFT) and
@@ -429,6 +431,90 @@ class OnlineTangoStream(_Geometry):
     @property
     def closed(self):
         return self._closed
+
+    # ---------------------------------------------------------------- saving and resuming
+    def state(self, index=None):
+        """The session state (stream_state) of all B streams, or of stream `index` alone as a B = 1 state: host copies
+        of every tensor, so the stream continues exactly as if it had not been called.  A closed stream raises
+        ValueError."""
+        if self._closed:
+            raise ValueError("the stream is closed (flushed, or an earlier push failed): it has no state to save")
+        if index is None:
+            take = lambda x, dim=0: stream_state.host(x)
+        else:
+            if isinstance(index, bool) or not isinstance(index, (int, np.integer)) or not 0 <= index < self.B:
+                raise ValueError("index must be a stream in 0..%d, got %r" % (self.B - 1, index))
+            i = int(index)
+            take = lambda x, dim=0: None if x is None else stream_state.host(x.narrow(dim, i, 1))
+        B, J, lag = (self.B if index is None else 1), self._T // self.block, self.lag
+        blocks = range(J - min(J, lag), J)
+
+        def filters(g, Ws, d):
+            if not blocks:
+                return torch.zeros((B, 0, g.n, self.F, d), dtype=torch.complex64)
+            return take(torch.stack([Ws[j] for j in blocks], 1))
+
+        groups = []
+        for g in self._groups:
+            pair = lambda R: None if R is None else [take(R[0]), take(R[1])]
+            hs, hn = (take(h[0]) for h in g.hist_sn) if self.clean else (None, None)
+            Sb, Nb = (take(b) for b in g.SNblk) if g.SNblk is not None else (None, None)
+            groups.append({"C": g.C, "nodes": list(g.nodes), "hist": take(g.hist[0]), "hist_s": hs, "hist_n": hn,
+                           "Yblk": take(g.Yblk), "Sblk": Sb, "Nblk": Nb, "R1": pair(g.R1), "R2": pair(g.R2),
+                           "W1": filters(g, g.W1s, g.C), "W2": filters(g, g.W2s, g.D)})
+        carry = take(self._carry, 1).transpose(0, 1).contiguous() if self.clean else take(self._carry).unsqueeze(1)
+        zs, zn = (take(b) for b in self._zsnblk) if self._zsnblk is not None else (None, None)
+        return {"version": stream_state.VERSION, "kind": "clean" if self.clean else "plain",
+                "n_fft": self.n_fft, "lambda_cor": self.lambda_cor, "block": self.block, "lag": lag, "mu": self.mu,
+                "rank": self.rank, "ref_mic": self.ref_mic, "filter_type": self.filter_type,
+                "mask_for_z": self.mask_for_z, "clean": self.clean, "vads": self.vads, "wide": self.D > 8,
+                "K": self.K, "C": self.C if self.channels is None else None,
+                "channels": None if self.channels is None else list(self.channels), "B": B,
+                "samples_in": self._L, "frames_out": self._T, "samples_out": self._S, "closed": J,
+                "groups": groups, "m1": take(self._m1), "m2": take(self._m2), "zblk": take(self._zblk),
+                "zsblk": zs, "znblk": zn, "carry": carry}
+
+    @classmethod
+    def from_state(cls, state, device=None):
+        """A stream that continues where `state` left off, on `device` (None: the current CUDA device).  A list of
+        states of identical options, geometry and counters makes one lockstep stream of B = sum(B_i) streams, in list
+        order; its outputs equal those of the streams the states came from when each stream's signals are paired
+        among themselves (n_C * C even for every channel-count group, and K even), as for online_tango_ragged's
+        batches (DESIGN §4.8).  ValueError for an invalid state or states that do not match, before any device work."""
+        st = stream_state.concat(state)
+        opts = {k: st[k] for k in ("n_fft", "lambda_cor", "block", "lag", "mu", "rank", "ref_mic")}
+        self = cls(st["B"], st["K"], st["C"] if st["channels"] is None else st["channels"], device=device,
+                   filter_type=st["filter_type"], mask_for_z=st["mask_for_z"], clean=st["clean"], vads=st["vads"],
+                   wide=st["wide"], **opts)
+        dev = lambda x: None if x is None else x.to(self.device, copy=True)
+        J = st["closed"]
+        for g, s in zip(self._groups, st["groups"]):
+            g.hist[0].copy_(s["hist"])
+            if self.clean:
+                g.hist_sn[0][0].copy_(s["hist_s"])
+                g.hist_sn[1][0].copy_(s["hist_n"])
+            g.Yblk.copy_(s["Yblk"])
+            if g.SNblk is not None:
+                g.SNblk[0].copy_(s["Sblk"])
+                g.SNblk[1].copy_(s["Nblk"])
+            g.R1 = None if s["R1"] is None else tuple(dev(r) for r in s["R1"])
+            g.R2 = None if s["R2"] is None else tuple(dev(r) for r in s["R2"])
+            nw = s["W1"].shape[1]
+            g.W1s = {J - nw + i: dev(s["W1"][:, i]).contiguous() for i in range(nw)}
+            g.W2s = {J - nw + i: dev(s["W2"][:, i]).contiguous() for i in range(nw)}
+        if self.clean:
+            self._carry.copy_(st["carry"].transpose(0, 1))
+        else:
+            self._carry.copy_(st["carry"][:, 0])
+        self._m1.copy_(st["m1"])
+        self._m2.copy_(st["m2"])
+        if self._zblk is not None:
+            self._zblk.copy_(st["zblk"])
+        if self._zsnblk is not None:
+            self._zsnblk[0].copy_(st["zsblk"])
+            self._zsnblk[1].copy_(st["znblk"])
+        self._L, self._T, self._S = st["samples_in"], st["frames_out"], st["samples_out"]
+        return self
 
     # ---------------------------------------------------------------- public calls
     def push(self, y_chunk, mask_fn=None, *, s_chunk=None, n_chunk=None):
@@ -668,6 +754,8 @@ class OnlineTangoPool(_Geometry):
         out = pool.push(y, n, mask_fn)   # y [S, K, C, n_max] float32 CUDA; slot s gets y[s, ..., :n[s]]
         out = pool.close(slots, mask_fn) # the last frame (reflected at the end), the partial block, the last samples
         pool.filters(slot)               # (W1 [K, F, C], W2 [K, F, D]) of the slot's last closed block, or None
+        st = pool.export(slot, release=False)   # the slot's session (stream_state); release=True frees the slot
+        pool.restore(slot, st)           # a free slot resumes a session of this pool's options and geometry
 
     For every slot, its outputs concatenated over the calls from open to close equal, value for value, those of
     OnlineTangoStream(1, K, C) with the same options fed the same samples (hence online_tango on the slot's whole
@@ -715,6 +803,7 @@ class OnlineTangoPool(_Geometry):
         self._S = np.zeros(S, dtype=np.int64)          # time samples out
         self._par = np.zeros(S, dtype=np.int64)        # which history buffer holds the slot's last n_fft samples
         self._nclosed = np.zeros(S, dtype=np.int64)    # closed blocks
+        self._seeded = np.zeros(S, dtype=bool)         # opened with R0: the carried matrices exist before a block
         self._bufs = False
 
     def _alloc(self):
@@ -806,6 +895,7 @@ class OnlineTangoPool(_Geometry):
             g.W1[i] = g.pass_[0]
             g.W2[i] = g.pass_[1]
         self._open[idx] = True
+        self._seeded[idx] = R0 is not None
         for a in (self._L, self._T, self._S, self._par, self._nclosed):
             a[idx] = 0
 
@@ -856,6 +946,93 @@ class OnlineTangoPool(_Geometry):
         out = self._run(chunk, np.zeros(self.S, dtype=np.int64), self._L.copy(), T1, S1, final, mask_fn)
         self._open[idx] = False
         return out
+
+    # ---------------------------------------------------------------- saving and moving sessions
+    def _one_slot(self, slot):
+        idx = self._slot_list([slot])
+        if len(idx) != 1:
+            raise ValueError("one slot, got %r" % (slot,))
+        return int(idx[0])
+
+    def export(self, slot, release=False):
+        """The session state (stream_state) of open slot `slot`: a B = 1 state in the format of
+        OnlineTangoStream.state(index), as host copies.  release=True frees the slot without emitting its tail; the
+        session lives on in the state."""
+        s = self._one_slot(slot)
+        if not self._open[s]:
+            raise ValueError("slot %d is not open" % s)
+        take = lambda x: stream_state.host(x[s:s + 1])
+        J, lag = int(self._nclosed[s]), self.lag
+        # the ring holds block j's filters at j % (lag + 1); the state keeps blocks J - nw .. J - 1
+        pos = torch.tensor([j % (lag + 1) for j in range(J - min(J, lag), J)], dtype=torch.int64)
+        groups = []
+        for g in self._groups:
+            R1 = None if J == 0 and not self._seeded[s] else [take(g.R1[0]), take(g.R1[1])]
+            R2 = None if J == 0 and (self.K > 1 or not self._seeded[s]) else [take(g.R2[0]), take(g.R2[1])]
+            groups.append({"C": g.C, "nodes": list(g.nodes), "hist": take(g.hist[int(self._par[s])]),
+                           "hist_s": None, "hist_n": None, "Yblk": take(g.Yblk), "Sblk": None, "Nblk": None,
+                           "R1": R1, "R2": R2, "W1": take(g.W1)[:, pos], "W2": take(g.W2)[:, pos]})
+        state = {"version": stream_state.VERSION, "kind": "plain",
+                 "n_fft": self.n_fft, "lambda_cor": self.lambda_cor, "block": self.block, "lag": lag, "mu": self.mu,
+                 "rank": self.rank, "ref_mic": self.ref_mic, "filter_type": self.filter_type,
+                 "mask_for_z": self.mask_for_z, "clean": False, "vads": None, "wide": self.D > 8,
+                 "K": self.K, "C": self.C if self.channels is None else None,
+                 "channels": None if self.channels is None else list(self.channels), "B": 1,
+                 "samples_in": int(self._L[s]), "frames_out": int(self._T[s]), "samples_out": int(self._S[s]),
+                 "closed": J, "groups": groups, "m1": take(self._m1), "m2": take(self._m2),
+                 "zblk": None if self._zblk is None else take(self._zblk), "zsblk": None, "znblk": None,
+                 "carry": take(self._carry).unsqueeze(1)}
+        if release:
+            self._open[s] = False
+        return state
+
+    def restore(self, slot, state):
+        """Open free slot `slot` from a B = 1 session state (stream_state): its later outputs from push and close
+        equal those the exporting stream or slot would have produced.  The state's options and geometry must be the
+        pool's, and it cannot hold clean components; ValueError before any change otherwise.  The state's tensors
+        are copied to the pool's device."""
+        s = self._one_slot(slot)
+        if self._open[s]:
+            raise ValueError("slot %d is already open" % s)
+        stream_state.check(state)
+        if state["B"] != 1:
+            raise ValueError("session state: B = %d: a slot takes one stream (OnlineTangoStream.state(index))"
+                             % state["B"])
+        if state["clean"]:
+            raise ValueError("session state: clean components cannot go into a pool (its slots take none)")
+        mine = {"n_fft": self.n_fft, "lambda_cor": self.lambda_cor, "block": self.block, "lag": self.lag,
+                "mu": self.mu, "rank": self.rank, "ref_mic": self.ref_mic, "filter_type": self.filter_type,
+                "mask_for_z": self.mask_for_z, "K": self.K, "C": self.C if self.channels is None else None,
+                "channels": None if self.channels is None else list(self.channels)}
+        for k, v in mine.items():
+            if state[k] != v:
+                raise ValueError("session state: %s is %r, the pool's %r" % (k, state[k], v))
+        self._alloc()
+        J, lag = state["closed"], self.lag
+        for g, st in zip(self._groups, state["groups"]):
+            g.hist[0, s].copy_(st["hist"][0])
+            g.Yblk[s].copy_(st["Yblk"][0])
+            for R, Rst in ((g.R1, st["R1"]), (g.R2, st["R2"])):
+                for w in range(2):
+                    if Rst is None:
+                        R[w][s] = 0                      # "none yet": the scan's R_(-1) is 0 either way
+                    else:
+                        R[w][s].copy_(Rst[w][0])
+            g.W1[s] = g.pass_[0]
+            g.W2[s] = g.pass_[1]
+            nw = st["W1"].shape[1]
+            for i in range(nw):
+                g.W1[s, (J - nw + i) % (lag + 1)].copy_(st["W1"][0, i])
+                g.W2[s, (J - nw + i) % (lag + 1)].copy_(st["W2"][0, i])
+        self._m1[s].copy_(state["m1"][0])
+        self._m2[s].copy_(state["m2"][0])
+        if self._zblk is not None:
+            self._zblk[s].copy_(state["zblk"][0])
+        self._carry[s].copy_(state["carry"][0, 0])
+        self._open[s] = True
+        self._seeded[s] = state["groups"][0]["R1"] is not None
+        self._L[s], self._T[s], self._S[s] = state["samples_in"], state["frames_out"], state["samples_out"]
+        self._par[s], self._nclosed[s] = 0, J
 
     # ---------------------------------------------------------------- internals
     def _slot_list(self, slots):
